@@ -11,6 +11,9 @@ Synthetic data: random-init weights of the named architecture, KV cache N(0,1) w
   roofline  dominant kernel (W4A16 gate_up_proj GEMV with the fused SiLU*mul epilogue - the variant the graph runs -
             28 launches/step): algorithmic bytes / launch duration, CUDA events around each launch in an instrumented
             pass; plus the paged decode attention kernel the north-star names, and the whole-step bytes/time
+  --dump-outputs DIR  after the timed steps, what the last timed step computed (logits as float32, greedy token ids as
+            float64) is written to DIR/<name>.npy, so that two builds can be compared output for output on the same
+            seeded inputs
   cpu_baseline  the oracle's restatement of one decoder layer (+ lm_head) on the host cores, bounded sample,
             median of >= 5 passes with the spread reported
   comparators   same-box library kernels (NOT the reference arm): FlashInfer fa2 decode / prefill (what the reference
@@ -42,7 +45,7 @@ if ROOT not in sys.path:
 METRIC = "decode_tokens_per_s"
 UNIT = "tokens/s"
 CTX = 4096
-WORKLOAD = "Qwen2-7B W4A16 (group 128), batch=1, ctx=4096, decode-only PagedAttention, 1xB200 per replica"
+WORKLOAD = "Qwen2-7B W4A16 (group 128), batch=1, ctx=4096, decode-only PagedAttention, 1xH100 per replica"
 
 
 def load_peaks():
@@ -50,26 +53,7 @@ def load_peaks():
         p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
-
-
-def profiled_traffic(name):
-    """DRAM bytes (read + write) per launch from a committed `ncu --set full` summary (profiles/, written by
-    tools/ncu_summary.py) of the SAME kernel variant and shape.  A cross-reference, not a live measurement: the key
-    `traffic_source` names the file so a stale summary is visible.  None when the summary is absent."""
-    unit = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    try:
-        for ln in open(os.path.join(ROOT, "profiles", name)):
-            if ln.startswith("traffic = dram read + write ="):
-                parts = ln.split("=")[-1].split("+")
-                total = 0.0
-                for part in parts:
-                    v, u = part.split()
-                    total += float(v) * unit[u]
-                return int(total)
-    except Exception:
-        pass
-    return None
+        return 3350.0, "fallback (H100 SXM data sheet HBM3 bandwidth)"
 
 
 class ClockSampler:
@@ -436,6 +420,8 @@ def main():
     ap.add_argument("--tp", type=int, default=0, help="tensor-parallel degree (default: min(N, 4) for Qwen2-7B's 28 heads)")
     ap.add_argument("--exchange", default="peer", choices=["peer", "nccl"])
     ap.add_argument("--no-scale-target", action="store_true", help="skip the Llama-3-70B FP8 batch-32 ctx-8192 measurement")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the logits and token ids of the last timed step to DIR/<name>.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -539,6 +525,11 @@ def main():
     ms = e0.elapsed_time(e1)
     log(f"timed region done: {ms:.1f} ms")
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        import numpy as np
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "logits.npy"), runner.logits.float().cpu().numpy())
+        np.save(os.path.join(args.dump_outputs, "next_tokens.npy"), runner.next_tokens.cpu().numpy().astype(np.float64))
     # a graph replay does not pass through the library's launch counter: count the kernels in one step eagerly
     n0 = _lib.launch_count()
     runner.launch_step()
@@ -590,7 +581,7 @@ def main():
     at_bytes = 2 * ctx * runner.nkv * cfg.head_dim * 2 + 2 * runner.nh * cfg.head_dim * 2 + 4 * npg
 
     # ---- prefill half of the metric (BASELINE.json: "... + prefill TFLOPS"): one decoder layer of the chunked-prefill
-    # shape of configs[2] (4 prompts x 2048 tokens per chunk): the four W4A16 tcgen05 GEMMs + causal prefill attention ----
+    # shape of configs[2] (4 prompts x 2048 tokens per chunk): the four W4A16 wgmma GEMMs + causal prefill attention ----
     prefill = None
     comparators = None
     if rank == 0 and tp == 1:
@@ -620,7 +611,7 @@ def main():
             try:
                 tf_peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["bf16_tflops_sustained"])
             except Exception:
-                tf_peak = 1400.0
+                tf_peak = 989.0             # H100 SXM data sheet, dense bf16
             prefill = {"workload": "one Qwen2-7B decoder layer, chunk of 4 x 2048 tokens (W4A16 linears + causal attention)",
                        "linear_tflops": gflop / tg / 1e12, "linear_frac_of_bf16_sustained": gflop / tg / 1e12 / tf_peak,
                        "attention_tflops_causal": aflop / ta / 1e12, "layer_tflops": (gflop + aflop) / (tg + ta) / 1e12,
@@ -656,7 +647,6 @@ def main():
             tps, step_s, threads, sample, spread = cpu_layer_baseline(budget_s=15.0)
             cpu = {"value": tps, "unit": UNIT, "cores": threads, "kind": "port", "sample": sample, "spread": spread}
         ach = gu_bytes / gu_us_avg / 1e3
-        traffic_file = "r02_w4_gemv_gateup.md"
         line = {
             "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": ms / args.steps, "higher_is_better": True,
@@ -678,9 +668,6 @@ def main():
                          "kernel": f"linear_w4a16_small_m_kernel{' + SiLU*mul epilogue' if fused_act else ''} "
                                    f"(gate_up_proj {gu_N}x{gu_K}, 28 launches/step)",
                          "per_rank": True, "achieved": ach, "peak": peak_gbs, "unit": "GB/s", "frac": ach / peak_gbs,
-                         # ncu dram__bytes_read+write of the same kernel variant and shape (single GPU, unsharded shape)
-                         "traffic": profiled_traffic(traffic_file) if tp == 1 else None,
-                         "traffic_source": f"profiles/{traffic_file} (committed ncu --set full summary; cross-reference)",
                          "peak_source": peak_src, "launch_us": gu_us_avg, "launch_us_median": gu_us_med,
                          "launch_us_chained": gu_us_chained, "bytes_per_launch": gu_bytes,
                          "method": "CUDA events around each of 2 x 28 launches (one per layer's weights: 1.9 GB > L2)",

@@ -1,7 +1,7 @@
 /*
  * xllm_b200_ops.h -- C-ABI of libxllm_b200_ops.so
  *
- * B200-native (sm_100a) replacement for the per-layer inference hot path of
+ * H100-native (sm_90a) replacement for the per-layer inference hot path of
  * jd-opensource/xllm (reference @ 87e8d6e, v0.9.0).  Every entry point takes
  * plain device pointers, sizes, element strides and a cudaStream_t (passed as
  * void*); none takes a torch type.  Each one cites the reference interface it
@@ -253,7 +253,7 @@ int xb_linear_w4a16_decode_fused(void* y, int64_t y_stride, const void* x, int64
 int xb_linear_w4a16_decode_fused_fits(int M, int K);
 /* additive (the reference has no weight-only kernel, SURVEY 8b-3).  Arithmetic form of the W4A16 decode kernels (M <= 8; group_size
  * 64 / 128), both defined in oracle/quant.py:
- *   0  bf16-weight form: w = bf16((q - z) * s) per weight, then the bf16 linear (what the tcgen05 prefill GEMM computes)
+ *   0  bf16-weight form: w = bf16((q - z) * s) per weight, then the bf16 linear (what the wgmma prefill GEMM computes)
  *   1  exact-dequant form: y = bf16(sum_g s_g * sum_{k in g} x_k (q_k - z_g) + b), fp32 - the integer nibbles go to the
  *      tensor core unscaled and scale / zero are applied once per (row, group); differs from form 0 only by the bf16
  *      rounding of w that form 0 makes (<= 2^-9 relative per weight).
@@ -264,7 +264,7 @@ int xb_set_w4_decode_form(int form);
  * spec oracle/quant.py with bits = 8: w = bf16((q - z) * s), y = bf16(sum_k f32(x) f32(w) + b).
  * qweight: tile-packed bytes [N/16][K/64][32 lanes][8 words] (xb_w8_pack_rows / quant.pack_w8): lane 4g+t holds rows
  * n0+g (words 0..3) and n0+g+8 (words 4..7), k in [k0+16t, k0+16t+16) ascending; meta [K/g][N] = bf16 scale | zero<<16.
- * xb_linear_w8a16_small_m: M <= 64 streaming kernel (decode); xb_gemm_w8a16: tcgen05 GEMM with the int8 -> bf16
+ * xb_linear_w8a16_small_m: M <= 64 streaming kernel (decode); xb_gemm_w8a16: wgmma GEMM with the int8 -> bf16
  * unpack fused into the MMA main loop (prefill). */
 int xb_linear_w8a16_small_m(void* y, int64_t y_stride, const void* x, int64_t x_stride,
                             const uint32_t* qweight, const uint32_t* meta, const void* bias,
@@ -292,7 +292,7 @@ int xb_act_and_mul_interleaved8_bf16(void* out, const void* input, int d, int nu
 /* additive, host-side packer (plain C, no CUDA; layout spec: oracle/quant.py, SURVEY 8b-3): q[N,K] uint8 (0..15) -> qweight tiles. */
 int xb_w4_pack_rows(uint32_t* qweight_out, const uint8_t* q, int N, int K);
 
-/* ---- K3 / K2: prefill and chunked-prefill attention (tcgen05 + TMEM + TMA) ---------------------------
+/* ---- K3 / K2: prefill and chunked-prefill attention (wgmma + TMA) ------------------------------------
  * ragged: replaces the FlashInfer `ragged_run` module behind xllm::kernel::cuda::batch_prefill
  *   (cuda_ops_api.h:52-66, batch_prefill.cpp:21-163): q [total_q, Hq, D], k/v [total_kv, Hkv, D] contiguous ragged,
  *   q_cu_seq_lens / kv_cu_seq_lens int32 [batch+1] on device, causal self-attention.
@@ -331,18 +331,15 @@ int xb_prefill_paged_split_bf16(const void* q, int64_t q_stride_n, int64_t q_str
 int64_t xb_prefill_split_workspace_bytes(int kv_splits, int64_t total_q, int num_qo_heads, int head_dim);
 int xb_prefill_plan_splits(int batch, int max_qo_len, int64_t max_kv_len, int num_qo_heads,
                            int num_kv_heads, int num_sms);
-/* Kernel variant of the prefill attention entry points (kv_splits == 1): 0 = one q tile per CTA, 1 = two q tiles per CTA
- * with two softmax warpgroups ping-ponging on the tensor core.  Same arithmetic ladder; returns the old variant. */
-int xb_set_prefill_variant(int variant);
 
-/* ---- tcgen05 GEMMs for prefill-sized M (any M; TMA zero-fills ragged edges) ---------------------
- * C[M,N] = A[M,K] . B[N,K]^T (+ bias), fp32 accumulation in TMEM, bf16 output.
+/* ---- wgmma GEMMs for prefill-sized M (any M; TMA zero-fills ragged edges) -----------------------
+ * C[M,N] = A[M,K] . B[N,K]^T (+ bias), fp32 accumulation in registers, bf16 output.
  * bf16:  replaces xllm::kernel::cuda::matmul (cuda_ops_api.h:167-169, matmul.cpp:20-24 -> F::linear).
  * fp8:   replaces xllm::kernel::cuda::cutlass_scaled_mm (cuda_ops_api.h:171-176,
  *        cutlass_w8a8/scaled_mm_entry.cu:55-108): a,b e4m3 [M,K] / [N,K] (b is the reference's b.t() view),
  *        C = a_scale * (b_scale * acc) (+ bias); scales fp32 with numel 1 (per-tensor) or M / N.
  * w4a16: the weight-only GEMM (SURVEY 8b-3): same packed operands as xb_linear_w4a16_small_m, int4->bf16
- *        unpack fused into the tcgen05 main loop. */
+ *        unpack fused into the wgmma main loop. */
 int xb_gemm_bf16(void* c, int64_t ldc, const void* a, int64_t lda, const void* b,
                  const void* bias, int M, int N, int K, xb_stream_t stream);
 int xb_gemm_fp8_scaled(void* c, int64_t ldc, const void* a_e4m3, int64_t lda,
@@ -352,12 +349,8 @@ int xb_gemm_fp8_scaled(void* c, int64_t ldc, const void* a_e4m3, int64_t lda,
 int xb_gemm_w4a16(void* c, int64_t ldc, const void* a, int64_t lda,
                   const uint32_t* qweight, const uint32_t* meta, const void* bias,
                   int M, int N, int K, int group_size, xb_stream_t stream);
-/* Kernel selection of the four xb_gemm_* entry points (tuning / tests; results are the same spec either way):
- * 0 = automatic, 1 = single-CTA kernels only, 2 = CTA-pair (tcgen05 cta_group::2, 256 x 256 tiles) kernels for shapes
- * with >= 74 pair tiles, 3 = CTA-pair kernels for every shape with M > 128 and N % 256 == 0.  Returns the old mode. */
-int xb_set_gemm_cta_pair(int mode);
 /* xb_gemm_fp8_scaled with M <= max_m (<= 64) runs swap-AB: the weight rows take the 128-row MMA M slot and the tokens the
- * N tile (what the reference's M <= 16 / M <= 64 buckets of scaled_mm_sm100_fp8_dispatch.cuh:148-287 do), so a
+ * N tile (what the reference's M <= 16 / M <= 64 buckets of its fp8 dispatch do), so a
  * decode-sized batch streams every weight tile on its own CTA.  0 = never.  Returns the old value. */
 int xb_set_fp8_swap_max_m(int max_m);
 /* split-K for the swap-AB FP8 GEMM: a decode-sized GEMM has only N/128 weight tiles (10 for a TP8 qkv shard of Llama-3-70B), so
@@ -371,8 +364,8 @@ int xb_set_gemm_splitk_workspace(void* ws, size_t bytes);
 /* host-only query (no device needed): k ranges xb_gemm_fp8_scaled uses for [M,K] x [N,K]^T on a device with sm_count SMs once a
  * workspace is registered (1 = unsplit): fill the SMs once, >= 12 k blocks of 128 per range, no empty range. */
 int xb_gemm_fp8_split_k(int M, int N, int K, int sm_count);
-/* host-only (no device needed): the kernel variant the tcgen05 GEMM entry points pick for a shape, as text ("bf16 pair 256x224",
- * "fp8 swap-AB bn=32 split_k=5", "w4 single bn=128").  kind: 0 bf16 | 1 fp8 | 2 w4a16 | 3 w8a16.  Returns the length, -1 on a bad
+/* host-only (no device needed): the kernel variant the GEMM entry points pick for a shape, as text ("bf16 bn=128",
+ * "fp8 swap-AB bn=32 split_k=5", "w4 bn=64").  kind: 0 bf16 | 1 fp8 | 2 w4a16 | 3 w8a16.  Returns the length, -1 on a bad
  * kind.  For capacity planning and the dispatch tests (tests/test_splitk_host_cpu.py). */
 int xb_gemm_describe(int kind, int M, int N, int K, int sm_count, char* buf, int buf_len);
 int xb_set_fp8_splitk_max(int max_split);   /* 1 = never split .. 32; default 8 (XB_FP8_SPLITK_MAX); returns the old value */

@@ -1,6 +1,6 @@
 """oracle/_ref: the reference's OWN elementwise CUDA kernels, compiled from the sources where they lie under /root/reference (nothing
 is copied into this repository): activation.cu, norm.cu, rope.cu, reshape_paged_cache.cu, fp8_quant.cu, fused_qknorm_rope.cu,
-moe/moe_fused_topk.cu, llm_decode_metadata_update.cu and fp8_scaled_quantize.cpp of xllm/core/kernels/cuda, with nvcc for sm_100a against the libtorch of this image.  They need no part of the reference's build system;
+moe/moe_fused_topk.cu, llm_decode_metadata_update.cu and fp8_scaled_quantize.cpp of xllm/core/kernels/cuda, with nvcc for sm_90a against the libtorch of this image.  They need no part of the reference's build system;
 the only missing header is <glog/logging.h>, for which oracle/ref_stubs/ forwards to c10's glog-compatible macros.  (Attention =
 FlashInfer and the FP8 GEMM = CUTLASS are un-vendored third-party code and stay "unbuildable": DESIGN.md section 2.)
 
@@ -51,7 +51,7 @@ def build(verbose=False, force=False):
         obj = os.path.join(OUT, "obj", os.path.basename(s).rsplit(".", 1)[0] + ".o")
         objs.append(obj)
         if force or not os.path.exists(obj):
-            jobs.append([NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-O2", "-std=c++17", "--expt-relaxed-constexpr",
+            jobs.append([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-O2", "-std=c++17", "--expt-relaxed-constexpr",
                          "--expt-extended-lambda", "-Xcompiler", "-fPIC", "-w"] + inc + ["-c", os.path.join(KDIR, s), "-o", obj])
 
     def run(cmd):
@@ -62,7 +62,7 @@ def build(verbose=False, force=False):
                 sys.stderr.write(" ".join(cmd) + "\n" + r.stdout[-4000:] + r.stderr[-4000:])
             if r.returncode != 0:
                 raise RuntimeError("reference kernel failed to compile: " + cmd[-3])
-    link = [NVCC, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", LIB] + objs + \
+    link = [NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", LIB] + objs + \
            [f"-L{ti}/lib", "-ltorch", "-ltorch_cpu", "-ltorch_cuda", "-lc10", "-lc10_cuda", f"-Xlinker=-rpath,{ti}/lib"]
     r = subprocess.run(link, capture_output=True, text=True)
     if r.returncode != 0:

@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on an H100 with `-m gpu`)")
     config.addinivalue_line("markers", "w4_exact: run with the exact-dequant form of the W4A16 decode kernels "
                                        "(xb_set_w4_decode_form(1)); every other GPU test pins the bf16-weight form")
 

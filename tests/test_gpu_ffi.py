@@ -96,6 +96,42 @@ def test_ffi_prefill_ragged_and_paged(built_lib):
     assert_close_attention(out2, ref2, scale2, what="FFI paged_run")
 
 
+def test_ffi_prefill_sm90_ragged_run(built_lib):
+    """the "_sm90" ragged-prefill module an sm90a device asks for (backend "fa3"): plan without the split arguments
+    (flashinfer_planinfo.cpp:119-137) and ragged_run with FlashInfer's FA3 argument list (batch_prefill.cpp:135-158)."""
+    import tvm_ffi
+    from xllm_b200 import build_ffi
+    ops_dir = build_ffi.build()
+    HQ, HKV, D = 28, 4, 128
+    uri = [u for u in build_ffi.uris_sm90() if f"head_dim_qk_{D}_" in u][0]
+    mod = tvm_ffi.load_module(os.path.join(ops_dir, uri, uri + ".so"))
+    g = torch.Generator().manual_seed(4)
+    lens = [300, 1, 777]
+    T = sum(lens)
+    qkv = torch.randn(T, (HQ + 2 * HKV) * D, generator=g).to(BF16)
+    cu = torch.tensor([0, 300, 301, 1078], dtype=torch.int32)
+    q = qkv[:, :HQ * D].reshape(T, HQ, D)
+    k = qkv[:, HQ * D:(HQ + HKV) * D].reshape(T, HKV, D)
+    v = qkv[:, (HQ + HKV) * D:].reshape(T, HKV, D)
+    sc = 1.0 / math.sqrt(D)
+    ws = torch.empty(1 << 20, dtype=torch.uint8, device=DEV)
+    pinned = torch.empty(1 << 20, dtype=torch.uint8).pin_memory()
+    d = qkv.to(DEV)
+    out = torch.empty(T, HQ, D, dtype=BF16, device=DEV)
+    lse = torch.empty(T, HQ, dtype=torch.float32, device=DEV)
+    with tvm_ffi.use_torch_stream():
+        plan = mod["plan"](ws, ws, pinned, cu, cu, torch.tensor(lens, dtype=torch.int32), T, len(lens), HQ, HKV, 1, False, D, D,
+                           True, -1)
+        mod["ragged_run"](ws, ws, plan, d[:, :HQ * D].view(T, HQ, D), d[:, HQ * D:(HQ + HKV) * D].view(T, HKV, D),
+                          d[:, (HQ + HKV) * D:].view(T, HKV, D), cu.to(DEV), cu.to(DEV), out, lse, 1, 0, -1, True,
+                          None, None, None, None, 0.0, sc, 1.0, 0)
+    torch.cuda.synchronize()
+    ref = O.ragged_prefill_attention(q, k, v, cu, cu, sc, causal=True)
+    scale = O.ragged_prefill_attention(q, k, v.abs(), cu, cu, sc, causal=True)
+    assert_close_attention(out, ref, scale, what="FFI sm90 ragged_run")
+    assert torch.isfinite(lse).all()
+
+
 def _ws():
     float_ws = torch.empty(128 << 20, dtype=torch.uint8, device=DEV)          # flashinfer_workspace.cpp:25-39 sizes
     int_ws = torch.empty(8 << 20, dtype=torch.uint8, device=DEV)

@@ -1,4 +1,4 @@
-"""GPU parity: tcgen05 GEMMs (bf16, FP8 W8A8, W4A16 dequant-GEMM) through the C ABI vs the oracle."""
+"""GPU parity: wgmma GEMMs (bf16, FP8 W8A8, W4A16 dequant-GEMM) through the C ABI vs the oracle."""
 import pytest
 import torch
 
@@ -19,7 +19,8 @@ def _abs_scale(x, w, b=None):
 
 # (M, N, K): tile-aligned, ragged M / N / K, multi-tile persistent, Qwen2-7B projections at chunk sizes
 BF16_SHAPES = [(128, 128, 64), (128, 128, 512), (256, 384, 1024), (100, 136, 200), (1, 64, 64), (333, 4608, 3584),
-               (2048, 3584, 3584), (512, 37888, 3584), (300, 3584, 18944), (129, 1152, 896)]
+               (2048, 3584, 3584), (512, 37888, 3584), (300, 3584, 18944), (129, 1152, 896), (256, 256, 64), (256, 256, 512),
+               (384, 512, 1024), (300, 768, 200), (1024, 3584, 3584), (2049, 4608, 3584), (256, 37888, 512)]
 
 
 @pytest.mark.parametrize("M,N,K", BF16_SHAPES)
@@ -62,7 +63,8 @@ def test_gemm_bf16_matches_small_m_kernel_bitwise_spec(built_lib):
 # reference's own test grid: tests/core/kernels/cuda/cutlass_scaled_mm_test.cpp:44-296 (up to 512x1024x768, per-tensor,
 # per-token x per-channel, bias) - there checked loosely (max diff < 2, mean < 0.5 vs fp32 matmul); here vs the oracle.
 FP8_CASES = [(16, 128, 128, False, False, False), (64, 256, 512, False, False, True), (512, 1024, 768, True, True, True),
-             (100, 272, 400, True, False, False), (300, 4608, 3584, False, True, True), (2048, 3584, 3584, False, False, False)]
+             (100, 272, 400, True, False, False), (300, 4608, 3584, False, True, True), (2048, 3584, 3584, False, False, False),
+             (300, 256, 400, True, False, False), (1024, 4608, 3584, True, True, False), (384, 37888, 3584, False, True, True)]
 
 
 @pytest.mark.parametrize("M,N,K,per_token,per_channel,use_bias", FP8_CASES)
@@ -117,7 +119,8 @@ def test_fp8_linear_static_and_dynamic(built_lib):
 
 
 W4_SHAPES = [(128, 128, 128), (64, 64, 64), (100, 192, 256), (333, 4608, 3584), (1024, 3584, 3584), (256, 37888, 3584),
-             (200, 3584, 18944), (17, 1152, 896)]
+             (200, 3584, 18944), (17, 1152, 896), (256, 256, 128), (300, 512, 256), (512, 37888, 3584), (400, 3584, 18944),
+             (1024, 4608, 3584)]
 
 
 @pytest.mark.parametrize("M,N,K", W4_SHAPES)
@@ -165,90 +168,11 @@ def test_w4a16_decode_and_prefill_kernels_agree(built_lib):
     assert_close_sum(y1, y2, _abs_scale(x.cpu(), wd), rtol=1e-5, what="w4 prefill vs decode kernel")
 
 
-# ---- CTA-pair (tcgen05 cta_group::2) variants: same spec, 256 x 256 tiles over two SMs --------------------------------
-@pytest.fixture
-def cta_pairs(built_lib):
-    from xllm_b200 import ops
-    old = ops.set_gemm_cta_pair(3)
-    yield
-    ops.set_gemm_cta_pair(old)
-
-
-PAIR_SHAPES = [(256, 256, 64), (256, 256, 512), (384, 512, 1024), (300, 768, 200), (1024, 3584, 3584), (512, 37888, 3584),
-               (2049, 4608, 3584)]
-
-
-@pytest.mark.parametrize("M,N,K", PAIR_SHAPES)
-def test_gemm_bf16_cta_pair(M, N, K, cta_pairs):
-    from xllm_b200 import ops
-    g = torch.Generator().manual_seed(2026)
-    a = torch.randn(M, K, generator=g).to(BF16)
-    w = (torch.randn(N, K, generator=g) * 0.02).to(BF16)
-    b = torch.randn(N, generator=g).to(BF16) if N % 3 == 0 else None
-    ref = O.linear(a, w, b)
-    ad, wd, bd = a.to(DEV), w.to(DEV), b.to(DEV) if b is not None else None
-    y = ops.gemm_bf16(ad, wd, bd)
-    assert_close_sum(y, ref, _abs_scale(a, w, b), rtol=1e-5, what=f"gemm_bf16 pair {M}x{N}x{K}")
-    assert_close_bf16(y, ref, ulps=1e9, rel_l2=1e-3, what="gemm_bf16 pair rel L2")
-    ops.set_gemm_cta_pair(1)
-    y1 = ops.gemm_bf16(ad, wd, bd)
-    ops.set_gemm_cta_pair(3)
-    assert_close_sum(y, y1, _abs_scale(a, w, b), rtol=1e-5, what="pair vs single-CTA kernel")
-
-
-@pytest.mark.parametrize("M,N,K,per_token,per_channel,use_bias", [(512, 1024, 768, True, True, True), (300, 256, 400 // 16 * 16, True, False, False),
-                                                                  (2048, 3584, 3584, False, False, False)])
-def test_cutlass_scaled_mm_cta_pair(M, N, K, per_token, per_channel, use_bias, cta_pairs):
-    from xllm_b200 import ops
-    g = torch.Generator().manual_seed(2026)
-    a = torch.randn(M, K, generator=g).clamp(-3, 3).to(E4M3)
-    w = torch.randn(N, K, generator=g).clamp(-3, 3).to(E4M3)
-    a_s = (torch.rand(M if per_token else 1, generator=g) * 0.1 + 0.01).float()
-    b_s = (torch.rand(N if per_channel else 1, generator=g) * 0.1 + 0.01).float()
-    bias = torch.randn(N, generator=g).to(BF16) if use_bias else None
-    ref = O.fp8_scaled_matmul(a, w, a_s, b_s, bias)
-    c = torch.empty(M, N, dtype=BF16, device=DEV)
-    ops.cutlass_scaled_mm(c, a.to(DEV), w.to(DEV).t(), a_s.to(DEV), b_s.to(DEV), bias.to(DEV) if bias is not None else None)
-    scale = (a.float().abs() @ w.float().abs().t()) * a_s.reshape(-1, 1) * b_s.reshape(1, -1)
-    if bias is not None:
-        scale = scale + bias.float().abs()
-    assert_close_sum(c, ref, scale, rtol=1e-5, what=f"cutlass_scaled_mm pair {M}x{N}x{K}")
-
-
-@pytest.mark.parametrize("M,N,K", [(256, 256, 128), (300, 512, 256), (1024, 3584, 3584), (512, 37888, 3584), (400, 3584, 18944)])
-def test_gemm_w4a16_cta_pair(M, N, K, cta_pairs):
-    from xllm_b200 import ops, quant
-    gs = 128
-    g = torch.Generator().manual_seed(2026)
-    w = (torch.randn(N, K, generator=g) * 0.02).to(BF16)
-    q, s, z = Q.quantize(w, 4, gs)
-    x = torch.randn(M, K, generator=g).to(BF16)
-    ref = Q.linear_wna16(x, q, s, z, gs, None)
-    qw, meta = quant.pack_w4(q, s, z, gs)
-    y = ops.gemm_w4a16(x.to(DEV), qw.to(DEV), meta.to(DEV), gs)
-    assert_close_sum(y, ref, _abs_scale(x, Q.dequantize(q, s, z, gs)), rtol=1e-5, what=f"gemm_w4a16 pair {M}x{N}x{K}")
-    assert_close_bf16(y, ref, ulps=1e9, rel_l2=1e-3, what="gemm_w4a16 pair rel L2")
-
-
-def test_gemm_w4a16_cta_pair_dequant_bit_exact(cta_pairs):
-    """identity activations read BOTH CTAs' dequantised halves of B back out of the pair MMA bit-for-bit."""
-    from xllm_b200 import ops, quant
-    g = torch.Generator().manual_seed(11)
-    N, K, gs = 512, 256, 128
-    w = torch.randn(N, K, generator=g).to(BF16)
-    q, s, z = Q.quantize(w, 4, gs)
-    wd = Q.dequantize(q, s, z, gs)
-    qw, meta = quant.pack_w4(q, s, z, gs)
-    x = torch.eye(K, dtype=BF16)
-    y = ops.gemm_w4a16(x.to(DEV), qw.to(DEV), meta.to(DEV), gs)
-    assert torch.equal(y.cpu(), wd.t().contiguous())
-
-
 @pytest.mark.parametrize("M,N,K,per_token,per_channel,use_bias", [(1, 256, 128, False, False, False), (32, 1280, 8192, True, True, True),
                                                                   (17, 8192, 1024, False, True, False), (64, 7168, 8192, True, False, True),
                                                                   (33, 1000, 416, False, False, False)])
 def test_cutlass_scaled_mm_swap_ab(M, N, K, per_token, per_channel, use_bias, built_lib):
-    """decode-sized M through the tcgen05 kernel with the weight rows in the MMA M slot (xb_set_fp8_swap_max_m): same spec."""
+    """decode-sized M through the wgmma kernel with the weight rows in the MMA M slot (xb_set_fp8_swap_max_m): same spec."""
     from xllm_b200 import ops
     g = torch.Generator().manual_seed(2026)
     a = torch.randn(M, K, generator=g).clamp(-3, 3).to(E4M3)

@@ -136,7 +136,7 @@ def test_interleave_index_is_a_permutation():
 @pytest.mark.parametrize("fmt", ["awq", "gptq"])
 def test_checkpoint_layout_tensor_through_the_kernels(fmt, built_lib):
     """SURVEY 8f n1 end to end on the GPU: tensors in the AutoAWQ / AutoGPTQ checkpoint layout -> from_awq / from_gptq ->
-    kernel layout (xb_w4_pack_rows) -> the decode GEMV and the tcgen05 dequant-GEMM, against the oracle on the logical form."""
+    kernel layout (xb_w4_pack_rows) -> the decode GEMV and the wgmma dequant-GEMM, against the oracle on the logical form."""
     from tests.test_checkpoint_surface import _logical, _pack_awq, _pack_seq_lastdim
     from xllm_b200 import ops, quant
     N, K, gs = 1152, 1024, 128

@@ -1,4 +1,4 @@
-"""GPU parity: prefill (ragged) and chunked-prefill (paged) attention on tcgen05 vs the oracle."""
+"""GPU parity: prefill (ragged) and chunked-prefill (paged) attention on wgmma vs the oracle."""
 import math
 
 import pytest
@@ -23,6 +23,7 @@ def _ragged_case(lens, HQ, HKV, D, seed=2026):
 RAGGED = [
     ([128], 28, 4, 128), ([128, 128], 16, 8, 128), ([32, 64, 128], 16, 8, 128), ([2048], 28, 4, 128),
     ([1, 5, 300, 17], 28, 4, 128), ([333, 700], 14, 2, 64), ([257], 8, 8, 128), ([513, 40], 32, 2, 128), ([130], 4, 4, 64),
+    ([2048, 2048], 28, 4, 128), ([4096], 32, 8, 128),
 ]
 
 
@@ -145,6 +146,6 @@ def test_chunked_prefill_split_kv_matches_oracle_and_unsplit(q_lens, kv_lens, pa
 def test_prefill_plan_splits_rule(built_lib):
     from xllm_b200 import ops
     assert ops.prefill_plan_splits(1, 2048, 2048, 28, 4) == 1          # 112 q tiles x 4 heads: plenty of CTAs
-    assert ops.prefill_plan_splits(1, 16, 8192, 28, 4) == 16           # 1 x 4 CTAs: min(148 / 4 = 37, 8192 / 512 = 16)
+    assert ops.prefill_plan_splits(1, 16, 8192, 28, 4) == 16           # 1 x 4 CTAs: min(132 / 4 = 33, 8192 / 512 = 16)
     assert ops.prefill_plan_splits(1, 16, 600, 28, 4) == 1             # short KV: not worth a merge pass
-    assert ops.prefill_plan_splits(8, 18, 4096, 28, 4) == 4            # 8 x 4 = 32 CTAs -> 148 / 32 = 4
+    assert ops.prefill_plan_splits(8, 18, 4096, 28, 4) == 4            # 8 x 4 = 32 CTAs -> 132 / 32 = 4

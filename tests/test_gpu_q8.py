@@ -1,4 +1,4 @@
-"""GPU parity of the 8-bit linears: W8A16 weight-only (streaming decode kernel + tcgen05 dequant-GEMM, spec
+"""GPU parity of the 8-bit linears: W8A16 weight-only (streaming decode kernel + wgmma dequant-GEMM, spec
 oracle/quant.py with bits = 8) and the FP8 W8A8 small-M (swap-AB streaming) kernel behind cutlass_scaled_mm."""
 import pytest
 import torch
@@ -43,7 +43,7 @@ def test_linear_w8a16_small_m(M, N, K, sym, built_lib):
 
 def test_w8a16_dequant_is_bit_exact(built_lib):
     """identity activations read single weights back: every one of the 256 levels, zero points across the 8-bit range
-    and both kernels (streaming and tcgen05 converter) must reproduce bf16((q - z) * s) bit for bit."""
+    and both kernels (streaming and wgmma converter) must reproduce bf16((q - z) * s) bit for bit."""
     from xllm_b200 import ops, quant
     g = torch.Generator().manual_seed(11)
     N, K, gs = 256, 256, 128
@@ -62,7 +62,7 @@ def test_w8a16_dequant_is_bit_exact(built_lib):
         y = ops.w8a16_linear_small_m(x.to(DEV), qw, meta, gs)
         assert torch.equal(y.cpu(), wd[:, k0:k0 + 64].t().contiguous()), f"streaming kernel: dequant mismatch in k block {k0}"
     y = ops.gemm_w8a16(torch.eye(K, dtype=BF16).to(DEV), qw, meta, gs)
-    assert torch.equal(y.cpu(), wd.t().contiguous()), "tcgen05 converter: dequant mismatch"
+    assert torch.equal(y.cpu(), wd.t().contiguous()), "wgmma converter: dequant mismatch"
 
 
 @pytest.mark.parametrize("M,N,K", [(128, 4608, 3584), (333, 3584, 3584), (2048, 37888, 3584), (512, 3584, 18944), (17, 1152, 896),
@@ -78,7 +78,7 @@ def test_gemm_w8a16(M, N, K, built_lib):
     qw, meta = quant.pack_w8(q, s, z, gs)
     y = ops.gemm_w8a16(x.to(DEV), qw.to(DEV), meta.to(DEV), gs, b.to(DEV) if b is not None else None)
     wd = Q.dequantize(q, s, z, gs)
-    if M * N * K > 2e10:      # full size: against the bf16 tcgen05 GEMM on the dequantised weight (the CPU oracle takes minutes)
+    if M * N * K > 2e10:      # full size: against the bf16 wgmma GEMM on the dequantised weight (the CPU oracle takes minutes)
         ref = ops.gemm_bf16(x.to(DEV), wd.to(DEV), b.to(DEV) if b is not None else None).cpu()
     else:
         ref = Q.linear_wna16(x, q, s, z, gs, b)
@@ -106,7 +106,7 @@ def test_w8a16_decode_and_prefill_kernels_agree(built_lib):
 @pytest.mark.parametrize("per_row", [False, True])
 def test_fp8_small_m_matches_oracle(M, N, K, per_row, built_lib):
     """the streaming swap-AB kernel behind cutlass_scaled_mm at decode sizes (M <= 64) against the oracle's
-    fp8_scaled_matmul (scaled_mm_entry.cu:55-108 semantics) and against the tcgen05 FP8 GEMM on the same inputs."""
+    fp8_scaled_matmul (scaled_mm_entry.cu:55-108 semantics) and against the FP8 GEMM on the same inputs."""
     from xllm_b200 import ops
     if N * K > 5e7 and M not in (1, 32):
         pytest.skip("full size at M = 1 and 32")
@@ -123,7 +123,7 @@ def test_fp8_small_m_matches_oracle(M, N, K, per_row, built_lib):
     assert_close_sum(c, ref, scale, rtol=1e-5, what=f"fp8 small-M {M}x{N}x{K} per_row={per_row}")
     assert_close_bf16(c, ref, ulps=1e9, rel_l2=1e-3, what="fp8 small-M rel L2")
     if N % 64 == 0:
-        # the tcgen05 kernel on the same inputs (forced by calling the GEMM entry point directly)
+        # the wgmma kernel on the same inputs (forced by calling the GEMM entry point directly)
         from xllm_b200._lib import c_i32, c_i64, check, lib
         c2 = torch.empty_like(c)
         ad, bd, asd, bsd = a.to(DEV), b.to(DEV), a_s.to(DEV), b_s.to(DEV)
@@ -131,7 +131,7 @@ def test_fp8_small_m_matches_oracle(M, N, K, per_row, built_lib):
         check(lib().xb_gemm_fp8_scaled(ops._p(c2), c_i64(c2.stride(0)), ops._p(ad), c_i64(ad.stride(0)), ops._p(bd), ops._p(asd),
                                        c_i32(asd.numel()), ops._p(bsd), c_i32(bsd.numel()), ops._p(bi), c_i32(M), c_i32(N), c_i32(K),
                                        ops._stream()), "gemm_fp8_scaled")
-        assert_close_sum(c, c2, scale, rtol=1e-5, what="fp8 small-M vs tcgen05 GEMM")
+        assert_close_sum(c, c2, scale, rtol=1e-5, what="fp8 small-M vs wgmma GEMM")
 
 
 def test_fp8_small_m_exact_products(built_lib):
@@ -150,20 +150,16 @@ def test_fp8_small_m_exact_products(built_lib):
 
 
 @pytest.mark.parametrize("M,N,K", [(256, 256, 128), (300, 512, 256), (1024, 3584, 3584)])
-def test_gemm_w8a16_cta_pair(M, N, K, built_lib):
-    """the CTA-pair (tcgen05 cta_group::2) kind-W8 kernel: each CTA of the pair converts 128 of the 256 B rows."""
+def test_gemm_w8a16_prefill_shapes(M, N, K, built_lib):
+    """the kind-W8 wgmma kernel at prefill-sized M: converter warps dequantise the int8 tiles into the MMA's B stages."""
     from xllm_b200 import ops, quant
-    old = ops.set_gemm_cta_pair(3)
-    try:
-        gs = 128
-        g = torch.Generator().manual_seed(2026)
-        w = (torch.randn(N, K, generator=g) * 0.02).to(BF16)
-        q, s, z = Q.quantize(w, 8, gs)
-        x = torch.randn(M, K, generator=g).to(BF16)
-        qw, meta = quant.pack_w8(q, s, z, gs)
-        y = ops.gemm_w8a16(x.to(DEV), qw.to(DEV), meta.to(DEV), gs)
-        wd = Q.dequantize(q, s, z, gs)
-        ref = Q.linear_wna16(x, q, s, z, gs, None)
-        assert_close_sum(y, ref, _abs_scale(x, wd, None), rtol=1e-5, what=f"gemm_w8a16 pair {M}x{N}x{K}")
-    finally:
-        ops.set_gemm_cta_pair(old)
+    gs = 128
+    g = torch.Generator().manual_seed(2026)
+    w = (torch.randn(N, K, generator=g) * 0.02).to(BF16)
+    q, s, z = Q.quantize(w, 8, gs)
+    x = torch.randn(M, K, generator=g).to(BF16)
+    qw, meta = quant.pack_w8(q, s, z, gs)
+    y = ops.gemm_w8a16(x.to(DEV), qw.to(DEV), meta.to(DEV), gs)
+    wd = Q.dequantize(q, s, z, gs)
+    ref = Q.linear_wna16(x, q, s, z, gs, None)
+    assert_close_sum(y, ref, _abs_scale(x, wd, None), rtol=1e-5, what=f"gemm_w8a16 {M}x{N}x{K}")

@@ -38,8 +38,8 @@ def test_linear_w4a16_exact_form(M, N, K, sym, built_lib):
     scale = x.float().abs() @ wd.float().abs().t() + (b.float().abs() if b is not None else 0)
     # (a) the form's own oracle.  The kernel accumulates sum x (128 + q) and subtracts (128 + z) sum x per group: its fp32
     # dot products run over terms |x| (128 + q) s, ~30x larger than |x||w|, so the honest fp32 bound (1e-5 of the sum of
-    # the magnitudes of the terms actually added, tests/util.py) is stated on THAT sum.  Measured on B200: up to 6e-5 of
-    # sum |x||w| at K = 18944 - the price of the form: about one bf16 ulp of a typical down_proj output.
+    # the magnitudes of the terms actually added, tests/util.py) is stated on THAT sum - the price of the form: about one
+    # bf16 ulp of a typical down_proj output.
     sg = s.float().repeat_interleave(gs, dim=1)
     scale_off = x.float().abs() @ ((q.float() + 128.0) * sg).t() + (b.float().abs() if b is not None else 0)
     assert_close_sum(y, Q.linear_wna16(x, q, s, z, gs, b, form="exact"), scale_off, rtol=1e-5, what=f"w4 exact M={M} N={N} K={K}")

@@ -1,7 +1,7 @@
-"""The shipped library really contains sm_100a tensor-core / TMA code (no GPU needed): cuobjdump of the in-tree
-libxllm_b200_ops.so must show the SASS forms of tcgen05.mma (UTCHMMA for bf16, UTCQMMA for fp8), TMEM loads (LDTM),
-TMA tensor loads / stores (UTMALDG / UTMASTG), mbarrier traffic (SYNCS) and the cp.async staging of the small-M kernels
-(LDGSTS) - in the kernels that are supposed to use them - and it must be built for sm_100a only."""
+"""The shipped library really contains sm_90a tensor-core / TMA code (no GPU needed): cuobjdump of the in-tree
+libxllm_b200_ops.so must show the SASS forms of wgmma (HGMMA), TMA tensor loads (UTMALDG),
+mbarrier traffic (SYNCS) and the cp.async staging of the small-M kernels (LDGSTS) - in the kernels that are supposed to
+use them - and it must be built for sm_90a only."""
 import re
 import shutil
 import subprocess
@@ -39,55 +39,38 @@ def _ops(sass, name_part):
     return sel
 
 
-def test_built_for_sm100a_only(built_lib):
+def test_built_for_sm90a_only(built_lib):
     out = subprocess.run([CUOBJDUMP, "-lelf", built_lib], capture_output=True, text=True).stdout
     archs = set(re.findall(r"sm_\d+a?", out))
-    assert archs == {"sm_100a"}, archs
+    assert archs == {"sm_90a"}, archs
 
 
-def test_gemm_kernels_use_tcgen05_tmem_tma(sass):
-    for name, ops in _ops(sass, "gemm_tcgen05_kernel").items():
-        assert ops & {"UTCHMMA", "UTCQMMA"}, f"{name}: no tcgen05.mma"
-        assert "LDTM" in ops, f"{name}: no TMEM load in the epilogue"
+def test_gemm_kernels_use_wgmma_tma(sass):
+    kernels = _ops(sass, "gemm_wgmma_kernel")
+    for name, ops in kernels.items():
+        assert "HGMMA" in ops, f"{name}: no wgmma"
         assert "UTMALDG" in ops, f"{name}: no TMA tensor load"
-        # the 32-column instantiation exists only for the swap-AB decode path (transposed plain stores, no TMA store box)
-        if "ILi1ELi32E" not in name:
-            assert "UTMASTG" in ops, f"{name}: no TMA tensor store"
         assert "SYNCS" in ops, f"{name}: no mbarrier pipeline"
-        assert "HMMA" not in ops, f"{name}: legacy mma.sync in a tcgen05 kernel"
-    pair = [k for k in sass if "gemm_tcgen05_kernel" in k and k.endswith("ELi2EEEv14CUtensorMap_stS2_S2_S2_NS0_10GemmParamsE")]
-    assert pair, "CTA-pair (cta_group::2) GEMM instantiations must be in the library"
-    fp8 = [k for k in sass if "gemm_tcgen05_kernel" in k and "UTCQMMA" in set(sass[k])]
-    assert fp8, "the FP8 GEMM must issue kind::f8f6f4 MMAs (UTCQMMA)"
+        assert "HMMA" not in ops, f"{name}: legacy mma.sync in a wgmma kernel"
+    fp8 = [k for k in kernels if "gemm_wgmma_kernelILi1E" in k]
+    assert fp8, "the FP8 GEMM instantiations must be in the library"
+    for k in fp8:
+        # converter warps widen e4m3 to fp16 (exact) for the fp32-accumulating fp16 wgmma
+        assert "F2FP" in kernels[k], f"{k}: no e4m3 -> f16 conversion"
 
 
-def test_prefill_attention_uses_tcgen05(sass):
+def test_prefill_attention_uses_wgmma(sass):
     for name, ops in _ops(sass, "prefill_attention_kernel").items():
-        assert "UTCHMMA" in ops and "LDTM" in ops and "STTM" in ops, name   # S/O in TMEM, lazy O rescale
+        assert "HGMMA" in ops and "HMMA" not in ops, name            # S = Q K^T and O += P V both on wgmma
         assert "UTMALDG" in ops and "MUFU" in ops, name
-
-
-def test_pingpong_prefill_attention_uses_tcgen05(sass):
-    for name, ops in _ops(sass, "prefill_attention2_kernel").items():
-        assert "UTCHMMA" in ops and "LDTM" in ops and "STTM" in ops, name
-        assert "UTMALDG" in ops and "MUFU" in ops and "HMMA" not in ops, name
-
-
-def test_pair_gemm_uses_2cta_instructions(sass):
-    """cta_group::2 shows up as .2CTA variants of the MMA, the TMA load and the commit (UTCBAR ... MULTICAST)."""
-    import subprocess as sp
-    from xllm_b200 import build
-    fun = "_ZN2xb2tc19gemm_tcgen05_kernelILi0ELi256ELi1ELi2EEEv14CUtensorMap_stS2_S2_S2_NS0_10GemmParamsE"
-    out = sp.run([CUOBJDUMP, "-sass", "-fun", fun, build.LIB], capture_output=True, text=True).stdout
-    assert "UTCHMMA.2CTA" in out and "UTMALDG.2D.2CTA" in out and "UTCBAR.2CTA.MULTICAST" in out
 
 
 def test_streaming_kernels_shape(sass):
     # HBM-bound small-M kernels: register-resident mma.sync fragments; the W4 kernel stages through cp.async
     for name, ops in _ops(sass, "linear_w4a16_small_m_kernel").items():
         assert "HMMA" in ops and "LDGSTS" in ops and "DEPBAR" in ops, f"{name}: expected mma.sync + cp.async groups"
-        assert not (ops & {"UTCHMMA", "UTCQMMA"}), name
+        assert not (ops & {"HGMMA", "QGMMA"}), name
     for name, ops in _ops(sass, "paged_decode_kernel").items():
         assert "HMMA" in ops and "MUFU" in ops, name
     for name, ops in _ops(sass, "allreduce").items():
-        assert not (ops & {"HMMA", "UTCHMMA"}), name
+        assert not (ops & {"HMMA", "HGMMA"}), name

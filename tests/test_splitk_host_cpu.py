@@ -15,7 +15,7 @@ def L(built_lib):
 
 
 def test_split_k_of_the_llama70b_shards(L):
-    f = lambda M, N, K: L.xb_gemm_fp8_split_k(M, N, K, 148)
+    f = lambda M, N, K: L.xb_gemm_fp8_split_k(M, N, K, 132)
     assert f(32, 1280, 8192) == 5          # qkv TP8 shard: 10 tiles, 64 k blocks -> 5 ranges of 13 (64 / 12 caps it)
     assert f(32, 8192, 1024) == 1          # o_proj TP8 shard: 8 k blocks - splitting measured slower
     assert f(32, 8192, 2048) == 1          # o_proj TP4 shard
@@ -23,7 +23,7 @@ def test_split_k_of_the_llama70b_shards(L):
     assert f(32, 8192, 3584) == 2          # down TP8 shard: 64 tiles, 28 k blocks
     assert f(32, 8192, 28672) == 2         # down unsharded
     assert f(32, 57344, 8192) == 1         # gate_up unsharded: 448 tiles already fill the SMs
-    assert f(32, 10240, 8192) == 1         # qkv unsharded: 80 tiles, 2 x 80 > 148
+    assert f(32, 10240, 8192) == 1         # qkv unsharded: 80 tiles, 2 x 80 > 132
     assert f(65, 1280, 8192) == 1 and f(32, 64, 8192) == 1 and f(0, 1280, 8192) == 1     # not a swap-AB shape
 
 
@@ -44,7 +44,7 @@ def test_split_k_invariants(L):
             assert kb_per >= 12, "range shorter than the TMA ring needs"
 
 
-def _describe(L, kind, M, N, K, sms=148):
+def _describe(L, kind, M, N, K, sms=132):
     buf = ctypes.create_string_buffer(96)
     n = L.xb_gemm_describe(kind, M, N, K, sms, buf, 96)
     assert n > 0
@@ -52,23 +52,21 @@ def _describe(L, kind, M, N, K, sms=148):
 
 
 def test_gemm_dispatch_of_the_baseline_shapes(L):
-    """which tcgen05 variant the GEMM entry points pick (xb_gemm_describe, host-only).  Qwen2-7B prefill at M = 8192 (BASELINE
-    configs[2]): CTA pairs everywhere, 224-column tiles where 256 leaves the last wave of the 74 pairs 14 % empty (N = 3584);
-    decode-sized FP8 (configs[3] shards): swap-AB, split-K on the narrow shards."""
+    """which wgmma variant the GEMM entry points pick (xb_gemm_describe, host-only).  Qwen2-7B prefill at M = 8192 (BASELINE
+    configs[2]): 128-column tiles; decode-sized FP8 (configs[3] shards): swap-AB, split-K on the narrow shards."""
     BF16, FP8, W4, W8 = 0, 1, 2, 3
-    for kind, name in ((BF16, "bf16"), (FP8, "fp8"), (W4, "w4")):
-        assert _describe(L, kind, 8192, 4608, 3584) == f"{name} pair 256x256"        # qkv
-        assert _describe(L, kind, 8192, 37888, 3584) == f"{name} pair 256x256"       # gate_up: 148 tile columns
-        assert _describe(L, kind, 8192, 3584, 3584) == f"{name} pair 256x224"        # o
-        assert _describe(L, kind, 8192, 3584, 18944) == f"{name} pair 256x224"       # down
-    assert _describe(L, W8, 8192, 3584, 18944) == "w8 pair 256x256"                  # no 224 instantiation for int8 tiles
-    # too few 256-row tiles for the 74 pairs: single-CTA kernels, BLOCK_N picked so that the tiles cover the SMs
-    assert _describe(L, BF16, 300, 4608, 3584) == "bf16 single bn=64"
-    assert _describe(L, W4, 2048, 1000, 512) == "w4 single bn=64"                    # N % 128 != 0
-    assert _describe(L, BF16, 17, 152064, 3584) == "bf16 single bn=256"              # lm_head of a small batch
+    for kind, name in ((BF16, "bf16"), (FP8, "fp8"), (W4, "w4"), (W8, "w8")):
+        assert _describe(L, kind, 8192, 4608, 3584) == f"{name} bn=128"        # qkv
+        assert _describe(L, kind, 8192, 37888, 3584) == f"{name} bn=128"       # gate_up
+        assert _describe(L, kind, 8192, 3584, 3584) == f"{name} bn=128"        # o
+        assert _describe(L, kind, 8192, 3584, 18944) == f"{name} bn=128"       # down
+    # too few 128 x 128 tiles to cover the SMs: 64-column tiles
+    assert _describe(L, BF16, 300, 4608, 3584) == "bf16 bn=64"
+    assert _describe(L, W4, 2048, 1000, 512) == "w4 bn=64"                    # N % 128 != 0
+    assert _describe(L, BF16, 17, 152064, 3584) == "bf16 bn=128"              # lm_head of a small batch
     # Llama-3-70B FP8 decode, batch 32
     assert _describe(L, FP8, 32, 1280, 8192) == "fp8 swap-AB bn=32 split_k=5"        # qkv TP8 shard
     assert _describe(L, FP8, 64, 8192, 28672) == "fp8 swap-AB bn=64 split_k=2"       # down unsharded, batch 64
     assert _describe(L, FP8, 32, 57344, 8192) == "fp8 swap-AB bn=32 split_k=1"       # gate_up unsharded
-    assert _describe(L, FP8, 65, 8192, 8192) == "fp8 single bn=64"                   # above the swap-AB bucket
-    assert L.xb_gemm_describe(7, 1, 1, 1, 148, ctypes.create_string_buffer(8), 8) == -1
+    assert _describe(L, FP8, 65, 8192, 8192) == "fp8 bn=64"                          # above the swap-AB bucket
+    assert L.xb_gemm_describe(7, 1, 1, 1, 132, ctypes.create_string_buffer(8), 8) == -1

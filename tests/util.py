@@ -53,9 +53,8 @@ def assert_close_attention(got, ref, abs_scale, rtol: float = 2e-3, what: str = 
     1.66e-3).  On synthetic N(0,1) V the output o = sum p_j v_j has the same magnitude as the error-carrying sum, so ONE
     implementation of the reference ladder sits 1.66e-3 (relative L2) from the un-rounded result, and two independent
     implementations (different tile / split order => different running maxima => independent roundings) sit
-    sqrt(2) * 1.66e-3 = 2.35e-3 apart before the bf16 rounding of o itself.  Measured on B200: this kernel vs the oracle
-    2.1-2.8e-3, FlashInfer's CUDA-core decode (fp32 P) vs the oracle 2.1e-3, this kernel vs FlashInfer's tensor-core
-    decode 0.5-3.3e-3 - the reference's own two decode paths differ from each other by as much.  The single-implementation
+    sqrt(2) * 1.66e-3 = 2.35e-3 apart before the bf16 rounding of o itself; the reference's own two decode paths (CUDA-core
+    and tensor-core FlashInfer) differ from each other by as much.  The single-implementation
     distance is asserted separately against the fp32-P oracle (test_paged_decode_distance_from_exact_math).
 
     The same bound with rtol = 1e-5 is used for fp32-accumulated dot products (linears): two correct summation orders

@@ -15,8 +15,7 @@ FI_BASE = os.path.join(ROOT, "baseline", "_fi")
 
 def set_env():
     os.environ["FLASHINFER_WORKSPACE_BASE"] = FI_BASE
-    os.environ["FLASHINFER_CUDA_ARCH_LIST"] = "10.0a"
-    os.makedirs(FI_BASE, exist_ok=True)
+    os.environ["FLASHINFER_CUDA_ARCH_LIST"] = "9.0a"
 
 
 def specs(head_dims=(128, 64)):
@@ -32,6 +31,7 @@ def specs(head_dims=(128, 64)):
 
 def main():
     set_env()
+    os.makedirs(FI_BASE, exist_ok=True)
     dims = tuple(int(a) for a in sys.argv[1:]) or (128, 64)
     for s in specs(dims):
         print("building", s.name, flush=True)

@@ -1,5 +1,5 @@
 """Development probe: FP8 W8A8 linears at decode batch sizes (M = 32 tokens) - the shipped dispatch (tokens in the 128-row MMA M
-slot, tcgen05 BLOCK_N 64 / streaming kernel) against the tcgen05 kernel in swap-AB mode (weight rows in the M slot, tokens as a
+slot, wgmma BLOCK_N 64 / streaming kernel) against the wgmma kernel in swap-AB mode (weight rows in the M slot, tokens as a
 32 / 64-column N tile, transposed store: xb_set_fp8_swap_max_m).  Shapes: Llama-3-70B projections, unsharded and
 the TP8 shard.  us per call from CUDA-graph replay over rotating weight copies (> L2)."""
 import os
@@ -55,7 +55,7 @@ def main():
         ops.set_fp8_swap_max_m(old)
         err = float((y.float() - ref).abs().max() / ref.abs().max())
         print(f"{name:12s} N={N:6d} K={K:6d} M={M}: shipped dispatch {t_cur:7.2f} us ({nb / t_cur / 1e3 / PEAK:5.1%})  streaming {t_small:7.2f} us "
-              f"({nb / t_small / 1e3 / PEAK:5.1%})  swapped tcgen05 {t_swap:7.2f} us ({nb / t_swap / 1e3 / PEAK:5.1%})  rel err {err:.1e}", flush=True)
+              f"({nb / t_small / 1e3 / PEAK:5.1%})  swapped wgmma {t_swap:7.2f} us ({nb / t_swap / 1e3 / PEAK:5.1%})  rel err {err:.1e}", flush=True)
         del ws
 
 

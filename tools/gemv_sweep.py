@@ -101,7 +101,7 @@ def run(name, N, K, M=1, gs=128, heads=None):
 
 
 def run_q8(name, N, K, M):
-    """W8A16 and FP8 W8A8 streaming kernels, and the small-M / tcgen05 crossover of the three weight formats."""
+    """W8A16 and FP8 W8A8 streaming kernels, and the small-M / wgmma crossover of the three weight formats."""
     gs = 128
     copies = max(2, int(400e6 / (N * K)) + 1)
     x = torch.randn(M, K, device=DEV, dtype=BF16)
@@ -118,7 +118,7 @@ def run_q8(name, N, K, M):
     if M > 16:
         fns = [lambda i=i: ops.gemm_w8a16(x, w8[i][0], w8[i][1], gs, None, y) for i in range(copies)]
         t = graph_time(fns)
-        print(f"{name:8s} N={N:6d} K={K:6d} M={M:2d} w8a16 tcgen05 GEMM   graph {t:7.2f} us ({nb / t / 1e3 / PEAK:5.1%})", flush=True)
+        print(f"{name:8s} N={N:6d} K={K:6d} M={M:2d} w8a16 wgmma GEMM   graph {t:7.2f} us ({nb / t / 1e3 / PEAK:5.1%})", flush=True)
     del w8
     f8 = [torch.randn(N, K, device=DEV).clamp(-3, 3).to(torch.float8_e4m3fn) for _ in range(copies)]
     a8 = torch.randn(M, K, device=DEV).clamp(-3, 3).to(torch.float8_e4m3fn)
@@ -132,7 +132,7 @@ def run_q8(name, N, K, M):
                                                       ops._p(one), c_i32(1), ops._p(one), c_i32(1), ops._p(None), c_i32(M), c_i32(N),
                                                       c_i32(K), ops._stream()), "gemm_fp8") for i in range(copies)]
     t = graph_time(fns)
-    print(f"{name:8s} N={N:6d} K={K:6d} M={M:2d} fp8 tcgen05 GEMM      graph {t:7.2f} us ({nb / t / 1e3 / PEAK:5.1%})", flush=True)
+    print(f"{name:8s} N={N:6d} K={K:6d} M={M:2d} fp8 wgmma GEMM      graph {t:7.2f} us ({nb / t / 1e3 / PEAK:5.1%})", flush=True)
     del f8
     # W4 crossover
     ws = weights(N, K, gs, max(2, int(400e6 / (N * K / 2)) + 1))
@@ -143,7 +143,7 @@ def run_q8(name, N, K, M):
     if M > 16:
         fns = [lambda i=i: ops.gemm_w4a16(x, ws[i][0], ws[i][1], gs, None, y) for i in range(len(ws))]
         t = graph_time(fns)
-        print(f"{name:8s} N={N:6d} K={K:6d} M={M:2d} w4a16 tcgen05 GEMM   graph {t:7.2f} us ({nb / t / 1e3 / PEAK:5.1%})", flush=True)
+        print(f"{name:8s} N={N:6d} K={K:6d} M={M:2d} w4a16 wgmma GEMM   graph {t:7.2f} us ({nb / t / 1e3 / PEAK:5.1%})", flush=True)
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-"""xllm_b200: B200-native (sm_100a) implementation of xLLM's per-layer inference hot path.
+"""xllm_b200: H100-native (sm_90a) implementation of xLLM's per-layer inference hot path.
 
 The product is the C-ABI library `xllm_b200/lib/libxllm_b200_ops.so`
 (include/xllm_b200_ops.h).  This package is the host-side mirror of the

@@ -1,4 +1,4 @@
-"""Builds libxllm_b200_ops.so (sm_100a only) in-tree with nvcc.
+"""Builds libxllm_b200_ops.so (sm_90a only) in-tree with nvcc.
 
 No torch, no cmake: the product is a plain C-ABI shared library
 (include/xllm_b200_ops.h).  Objects are cached by source mtime under
@@ -15,7 +15,7 @@ LIBDIR = os.path.join(HERE, "lib")
 OBJDIR = os.path.join(LIBDIR, "obj")
 LIB = os.path.join(LIBDIR, "libxllm_b200_ops.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
          "-Xptxas", "-v" if os.environ.get("XB_PTXAS_V") else "-warn-spills"]
 

@@ -3,7 +3,8 @@ get_module(uri) (xllm/core/kernels/cuda/utils.cpp:371-374,526-564) loads them un
 
     $FLASHINFER_OPS_PATH/<uri>/<uri>.so      exporting __tvm_ffi_plan / __tvm_ffi_run | __tvm_ffi_{ragged,paged}_run
 
-One decode and one prefill module are compiled (g++, apache-tvm-ffi headers) against libxllm_b200_ops.so and installed
+One decode module, one prefill module and the FA3 form of the prefill module (the "_sm90" URIs the reference requests for
+ragged prefill on an sm90a device) are compiled (g++, apache-tvm-ffi headers) against libxllm_b200_ops.so and installed
 under every URI the reference can request for bf16 (utils.cpp:388-450), by symlink.
 """
 import os
@@ -26,6 +27,11 @@ def uris():
     return dec, pre
 
 
+def uris_sm90():
+    """the ragged-prefill URIs the reference requests on an sm90a device (backend "fa3": utils.cpp:376-386,417)"""
+    return [u + "_sm90" for u in uris()[1]]
+
+
 def build(verbose=False):
     import tvm_ffi
     root = os.path.dirname(tvm_ffi.__file__)
@@ -37,7 +43,8 @@ def build(verbose=False):
                 inc.append(cand)
     os.makedirs(OPS_DIR, exist_ok=True)
     outs = {}
-    for name, macro in (("xllm_b200_ffi_decode", ["-DXB_FFI_DECODE_MODULE"]), ("xllm_b200_ffi_prefill", [])):
+    for name, macro in (("xllm_b200_ffi_decode", ["-DXB_FFI_DECODE_MODULE"]), ("xllm_b200_ffi_prefill", []),
+                        ("xllm_b200_ffi_prefill_sm90", ["-DXB_FFI_PREFILL_SM90_MODULE"])):
         out = os.path.join(LIBDIR, name + ".so")
         cmd = ["g++", "-O2", "-std=c++17", "-fPIC", "-shared", SRC, "-o", out] + macro + [f"-I{i}" for i in inc] + [
             f"-L{LIBDIR}", "-lxllm_b200_ops", f"-L{os.path.join(root, 'lib')}", "-ltvm_ffi", "-L/usr/local/cuda/lib64", "-lcudart",
@@ -49,7 +56,8 @@ def build(verbose=False):
             raise RuntimeError("FFI module build failed")
         outs[name] = out
     dec, pre = uris()
-    for lst, so in ((dec, outs["xllm_b200_ffi_decode"]), (pre, outs["xllm_b200_ffi_prefill"])):
+    for lst, so in ((dec, outs["xllm_b200_ffi_decode"]), (pre, outs["xllm_b200_ffi_prefill"]),
+                    (uris_sm90(), outs["xllm_b200_ffi_prefill_sm90"])):
         for uri in lst:
             d = os.path.join(OPS_DIR, uri)
             os.makedirs(d, exist_ok=True)

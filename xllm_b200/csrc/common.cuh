@@ -1,4 +1,4 @@
-// Shared device/host helpers for libxllm_b200_ops (sm_100a only).
+// Shared device/host helpers for libxllm_b200_ops (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp8.h>
@@ -37,9 +37,8 @@ extern std::atomic<int> g_pdl_enabled;
   } while (0)
 
 // Experiment switch (OFF by default): XB_SMEM_CARVEOUT=1 makes every kernel ask for the maximum shared-memory carveout,
-// so that consecutive kernels of a decode step never re-partition the SM.  Measured on B200 it LOSES 11 % of the decode
-// step (567 -> 504 tok/s; paged decode 7.9 -> 10.0 us): the streaming kernels want the L1 that the driver's per-kernel
-// heuristic leaves them.
+// so that consecutive kernels of a decode step never re-partition the SM.  Off by default: the streaming kernels want the
+// L1 that the driver's per-kernel heuristic leaves them.
 void prefer_max_shared_carveout(const void* kernel);
 
 // Launch helper: counts launches, optionally attaches the PDL attribute.

@@ -9,7 +9,7 @@
 // Tensors arrive as borrowed DLPack views; the CUDA stream is the one the host bound with TVMFFIEnvSetStream
 // (utils.h:147-161).  Everything forwards to the C ABI of libxllm_b200_ops.so; plan_info is opaque to xLLM
 // (deep-copied only: flashinfer_planinfo.cpp:37-62), so it carries this library's own int64 layout.
-// Build: see xllm_b200/build_ffi.py (one .so, installed under the decode and the prefill URI directories).
+// Build: see xllm_b200/build_ffi.py (decode, prefill and FA3-form prefill modules, installed under their URI directories).
 #include <cuda_runtime.h>
 #include <tvm/ffi/container/array.h>
 #include <tvm/ffi/container/tensor.h>
@@ -50,7 +50,7 @@ void make_decode_plan(int64_t* plan, const TensorView& float_ws, const TensorVie
                       bool enable_cuda_graph) {
   int64_t max_pages = 1;
   for (int64_t b = 0; b < batch_size; ++b) max_pages = std::max<int64_t>(max_pages, indptr_host[b + 1] - indptr_host[b]);
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   if (enable_cuda_graph) {
@@ -120,7 +120,7 @@ void DecodeRun(TensorView float_ws, TensorView int_ws, Array<int64_t> plan_vec, 
 // ---------------------------------------------------------------------------------------------------------------
 // plan_info of the prefill module: [0] max_qo_len [1] batch [2] total rows [3] qo heads [4] causal
 //   [5] 1 = every request has exactly one query row: paged_run is served by the split-KV decode kernel, whose plan8
-//       follows in [6..13]; 0: [6] = kv_splits of the tcgen05 paged kernel (1 = no split)  (a one-row query sees the whole KV under either mask mode: FlashInfer masks
+//       follows in [6..13]; 0: [6] = kv_splits of the paged prefill kernel (1 = no split)  (a one-row query sees the whole KV under either mask mode: FlashInfer masks
 //       kv_idx + qo_len > kv_len + q_idx, prefill.cuh:1017)
 Array<int64_t> PrefillPlan(TensorView float_ws, TensorView int_ws, TensorView pinned_int_ws, TensorView qo_indptr_host,
                            TensorView kv_indptr_host, TensorView kv_len_arr_host, int64_t total_num_rows, int64_t batch_size,
@@ -151,7 +151,7 @@ Array<int64_t> PrefillPlan(TensorView float_ws, TensorView int_ws, TensorView pi
     const int32_t* kvl = static_cast<const int32_t*>(ptr(kv_len_arr_host));
     int64_t max_kv = 0;
     for (int64_t b = 0; b < batch_size; ++b) max_kv = std::max<int64_t>(max_kv, kvl[b]);
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int splits = (disable_split_kv || page_size <= 1) ? 1
@@ -253,6 +253,34 @@ void PagedRun(TensorView float_ws, TensorView int_ws, Array<int64_t> plan_vec, T
            "batch prefill paged_run");
 }
 
+// FA3 form of the ragged prefill module.  On an sm90a device the reference picks backend "fa3" for ragged prefill
+// (utils.cpp:376-386), requests the URI with the "_sm90" suffix (utils.cpp:417), calls `plan` without fixed_split_size /
+// disable_split_kv / num_colocated_ctas (flashinfer_planinfo.cpp:119-137) and `ragged_run` with FlashInfer's FA3 argument
+// list (batch_prefill.cpp:129-158).  Both route to the same kernels as the fa2 entry points.
+Array<int64_t> PrefillPlanSm90(TensorView float_ws, TensorView int_ws, TensorView pinned_int_ws, TensorView qo_indptr_host,
+                               TensorView kv_indptr_host, TensorView kv_len_arr_host, int64_t total_num_rows,
+                               int64_t batch_size, int64_t num_qo_heads, int64_t num_kv_heads, int64_t page_size,
+                               bool enable_cuda_graph, int64_t head_dim_qk, int64_t head_dim_vo, bool causal,
+                               int64_t window_left) {
+  return PrefillPlan(float_ws, int_ws, pinned_int_ws, qo_indptr_host, kv_indptr_host, kv_len_arr_host, total_num_rows,
+                     batch_size, num_qo_heads, num_kv_heads, page_size, enable_cuda_graph, head_dim_qk, head_dim_vo, causal,
+                     window_left, -1, false, 0);
+}
+
+void RaggedRunSm90(TensorView float_ws, TensorView int_ws, Array<int64_t> plan_vec, TensorView q, TensorView k, TensorView v,
+                   TensorView qo_indptr, TensorView kv_indptr, TensorView o, Optional<TensorView> maybe_lse,
+                   int64_t mask_mode_code, int64_t layout, int64_t window_left, bool enable_pdl,
+                   Optional<TensorView> maybe_prefix_len_ptr, Optional<TensorView> maybe_token_pos_in_items_ptr,
+                   Optional<TensorView> maybe_max_item_len_ptr, Optional<TensorView> maybe_scale_v, double logits_soft_cap,
+                   double sm_scale, double scale_v_scalar, int64_t token_pos_in_items_len) {
+  // scale_v exists for fp8 K/V (batch_prefill.cpp:130-133); with bf16 K/V the reference passes no tensor and 1.0
+  if (maybe_scale_v.has_value() || scale_v_scalar != 1.0) TVM_FFI_THROW(ValueError) << "fp8 V scaling is not implemented";
+  RaggedRun(float_ws, int_ws, plan_vec, q, k, v, qo_indptr, kv_indptr, o, maybe_lse, mask_mode_code, layout, window_left,
+            enable_pdl, Optional<TensorView>(), Optional<TensorView>(), Optional<TensorView>(), maybe_prefix_len_ptr,
+            maybe_token_pos_in_items_ptr, maybe_max_item_len_ptr, logits_soft_cap, sm_scale, 1.0, 1.0 / 10000.0,
+            token_pos_in_items_len);
+}
+
 // Optional capability probe (integration/patches/0003): a decode plan made under enable_cuda_graph depends only on the
 // captured (padded) batch and the workspace sizes - the kernels derive the split geometry on the device from the live paged
 // triplet and the arrival counters reset themselves - so a CUDA-graph executor may plan once and skip the host-side plan
@@ -262,9 +290,12 @@ int64_t PlanIsReplayInvariant() { return 1; }
 }  // namespace
 
 TVM_FFI_DLL_EXPORT_TYPED_FUNC(plan_is_replay_invariant, PlanIsReplayInvariant);
-#ifdef XB_FFI_DECODE_MODULE
+#if defined(XB_FFI_DECODE_MODULE)
 TVM_FFI_DLL_EXPORT_TYPED_FUNC(plan, DecodePlan);
 TVM_FFI_DLL_EXPORT_TYPED_FUNC(run, DecodeRun);
+#elif defined(XB_FFI_PREFILL_SM90_MODULE)
+TVM_FFI_DLL_EXPORT_TYPED_FUNC(plan, PrefillPlanSm90);
+TVM_FFI_DLL_EXPORT_TYPED_FUNC(ragged_run, RaggedRunSm90);
 #else
 TVM_FFI_DLL_EXPORT_TYPED_FUNC(plan, PrefillPlan);
 TVM_FFI_DLL_EXPORT_TYPED_FUNC(ragged_run, RaggedRun);

@@ -7,7 +7,7 @@
 //     weight: qweight8[N/16][K/64][32 lanes][8 words]; lane (g,t) owns rows n0+g (words 0..3) and n0+g+8 (words 4..7),
 //     k in [k0+16t, k0+16t+16), bytes ascending in k.  meta[K/g][N] = bf16 scale | zero << 16.  Dequant per 4 weights:
 //     4 PRMT + 4 FADD + 2 CVT.BF16X2 + 2 HMUL2.BF16 (bit-exact, see w8_dequant_word), 4 legacy HMMAs per k64 tile.
-//     The same packed tensor feeds the tcgen05 prefill GEMM (gemm_tcgen05.cu kind W8).
+//     The same packed tensor feeds the wgmma prefill GEMM (gemm_wgmma.cu kind W8).
 //
 //  FP8 W8A8 (fp8_linear_forward, xllm/core/layers/common/linear.cpp:137-182 -> cutlass_scaled_mm,
 //  kernels/cuda/cutlass_w8a8/scaled_mm_entry.cu:55-108; the reference buckets M <= 16 / <= 64 into swap-AB tiles,
@@ -205,7 +205,7 @@ linear_fp8_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, const
       float s = 0.f;
 #pragma unroll
       for (int ww = 0; ww < kQ8Warps; ++ww) s += red[ww][m][r * 8 + c];
-      // same order as the tcgen05 FP8 GEMM epilogue and the oracle: a_s * (b_s * acc) + bias
+      // same order as the FP8 GEMM epilogue and the oracle: a_s * (b_s * acc) + bias
       const float as = a_scale[a_per_row ? tok : 0], bs = b_scale[b_per_col ? n : 0];
       float v = as * (bs * s);
       if (bias) v += __bfloat162float(bias[n]);
@@ -222,7 +222,7 @@ extern "C" int xb_linear_w8a16_small_m(void* y, int64_t y_stride, const void* x,
                                        const uint32_t* meta, const void* bias, int M, int N, int K, int group_size,
                                        xb_stream_t stream) {
   if (M == 0) return 0;
-  XB_CHECK(M > 0 && M <= 64, "linear_w8a16_small_m: M=%d out of range (1..64); use the tcgen05 GEMM", M);
+  XB_CHECK(M > 0 && M <= 64, "linear_w8a16_small_m: M=%d out of range (1..64); use the wgmma GEMM", M);
   XB_CHECK(N % 16 == 0 && K % 64 == 0, "linear_w8a16_small_m: N=%d must be %%16, K=%d %%64", N, K);
   XB_CHECK(group_size >= 64 && group_size % 64 == 0 && K % group_size == 0,
            "linear_w8a16_small_m: group_size %d must be a multiple of 64 dividing K=%d", group_size, K);
@@ -261,7 +261,7 @@ extern "C" int xb_linear_fp8_small_m(void* c, int64_t ldc, const void* a, int64_
                                      int a_scale_numel, const float* b_scale, int b_scale_numel, const void* bias, int M,
                                      int N, int K, xb_stream_t stream) {
   if (M == 0 || N == 0) return 0;
-  XB_CHECK(M > 0 && M <= 64, "linear_fp8_small_m: M=%d out of range (1..64); use the tcgen05 GEMM", M);
+  XB_CHECK(M > 0 && M <= 64, "linear_fp8_small_m: M=%d out of range (1..64); use the wgmma GEMM", M);
   XB_CHECK(K % 64 == 0 && lda % 16 == 0, "linear_fp8_small_m: K=%d / lda=%lld must be multiples of 64 / 16", K, (long long)lda);
   XB_CHECK(((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b)) & 15) == 0, "linear_fp8_small_m: a / b not 16B aligned");
   XB_CHECK(a_scale_numel == 1 || a_scale_numel == M, "linear_fp8_small_m: a_scales must have numel 1 or M");

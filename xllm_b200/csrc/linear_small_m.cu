@@ -13,7 +13,7 @@
 //   (q | 0x4300) is bf16(128+q) exactly; (128+q)-(128+z) is exact; one rounding
 //   in the multiply by s.
 //
-// Tile-packed W4 layout (shared with the tcgen05 prefill GEMM, which writes the
+// Tile-packed W4 layout (shared with the wgmma prefill GEMM, which writes the
 // same per-thread 16-element k runs as 16-byte swizzled smem chunks):
 //   qweight[N/16][K/64][lane 0..31][word 0..3]  (uint32)
 //   lane = 4*g + t owns rows n0+g and n0+g+8, k in [k0+16t, k0+16t+16).
@@ -80,8 +80,8 @@ __device__ __forceinline__ XFrag load_x(const __nv_bfloat16* x, int64_t x_stride
 // register ring of kDepth slots (one slot = kTG k64 tiles = kTG 16-byte loads + the group's scale/zero
 // words) that is refilled as it is consumed: the HBM pipe never drains between tiles.  kSplit warps of a
 // CTA share a row tile and reduce through shared memory; with kSplit == 1 (wide N, e.g. gate_up) a warp
-// owns its rows outright and writes them directly.  The inner loop is instruction-bound next to HBM on
-// B200 (5.5 lane-ops per HBM byte): addresses are running pointers, the group index is a shift, and the
+// owns its rows outright and writes them directly.  The inner loop runs several lane-ops per HBM byte, so it is
+// instruction-bound next to HBM: addresses are running pointers, the group index is a shift, and the
 // per-weight work is exactly LOP3(+SHF) / HSUB2 / HMUL2 per bf16 PAIR plus one HMMA per 8 weights.
 // ---------------------------------------------------------------------------
 template <int kMT>
@@ -157,7 +157,7 @@ linear_w4a16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, con
   const int s_end = live ? min(nslots, s_begin + per) : s_begin;
 
   // kAcc independent accumulator sets (one per k16 step of a tile when registers allow): legacy HMMA has a long
-  // issue-to-result latency on sm_100, a single chain per warp leaves the scheduler with nothing eligible
+  // issue-to-result latency, a single chain per warp leaves the scheduler with nothing eligible
   constexpr int kAcc = kMT == 1 ? 4 : (kMT == 2 ? 2 : 1);
   float accj[kAcc][kMT][4];
 #pragma unroll
@@ -713,7 +713,7 @@ static int w4_small_m_impl(void* y, int64_t y_stride, const void* x, int64_t x_s
                            const uint32_t* meta, const void* bias, int M, int N, int K, int group_size, int epi,
                            int act_mode, bool xs, const W4Fuse* fzp, xb_stream_t stream) {  // (xs is forced on by the exact form)
   if (M == 0) return 0;
-  XB_CHECK(M > 0 && M <= 64, "linear_w4a16_small_m: M=%d out of range (1..64); use the tcgen05 GEMM", M);
+  XB_CHECK(M > 0 && M <= 64, "linear_w4a16_small_m: M=%d out of range (1..64); use the wgmma GEMM", M);
   XB_CHECK(N % 16 == 0 && K % 64 == 0, "linear_w4a16_small_m: N=%d must be %%16, K=%d %%64", N, K);
   XB_CHECK(group_size >= 64 && group_size % 64 == 0 && K % group_size == 0,
            "linear_w4a16_small_m: group_size %d must be a multiple of 64 dividing K=%d", group_size, K);
@@ -727,10 +727,11 @@ static int w4_small_m_impl(void* y, int64_t y_stride, const void* x, int64_t x_s
   auto* qw = reinterpret_cast<const uint4*>(qweight);
   auto* bb = reinterpret_cast<const __nv_bfloat16*>(bias);
   cudaStream_t s = (cudaStream_t)stream;
-  // pick the k split so that (row tiles x splits) covers ~16 warps on each of the 148 SMs
+  // pick the k split so that (row tiles x splits) covers ~16 warps on each of the device's SMs
   const int ntiles = N / 16, ktiles = K / 64;
   int split = 1;
-  while (split < 8 && ntiles * split < 148 * 16 && ktiles / (split * 2) >= 3) split *= 2;
+  static const int sms = [] { int d = 0, n = 132; cudaGetDevice(&d); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d); return n; }();
+  while (split < 8 && ntiles * split < sms * 16 && ktiles / (split * 2) >= 3) split *= 2;
   if (epi == 3 && split < 2) split = 2;   // the residual + statistics epilogue lives in the k-split reduction
   const int tpg = group_size / 64;   // k64 tiles per quantisation group
   XB_CHECK((tpg & (tpg - 1)) == 0, "linear_w4a16_small_m: group_size/64 must be a power of two (got %d)", group_size);
@@ -743,7 +744,6 @@ static int w4_small_m_impl(void* y, int64_t y_stride, const void* x, int64_t x_s
                      w4_xs_bytes(M, K) + w4_gsum_bytes(K, group_size) <= kXsMaxBytes;
   if (exact) xs = true;
   const size_t xs_bytes = (xs ? w4_xs_bytes(M, K) : 0) + (exact ? w4_gsum_bytes(K, group_size) : 0);
-  // (tuning note, B200: 3 CTAs/SM at <= 80 registers measured 10-13 % slower than 2 CTAs/SM for every decode shape)
 #define XB_W4_GO(MT, SP, DEPTH, TG, EPI, XS, EX)                                                                   \
   {                                                                                                                 \
     auto kern = linear_w4a16_small_m_kernel<MT, SP, DEPTH, TG, 2, EPI, XS, EX>;                                     \
@@ -902,7 +902,7 @@ extern "C" int xb_linear_w4a16_decode_fused_fits(int M, int K) {
 extern "C" int xb_linear_bf16_small_m(void* y, int64_t y_stride, const void* x, int64_t x_stride, const void* w,
                                       const void* bias, int M, int N, int K, xb_stream_t stream) {
   if (M == 0) return 0;
-  XB_CHECK(M > 0 && M <= 64, "linear_bf16_small_m: M=%d out of range (1..64); use the tcgen05 GEMM", M);
+  XB_CHECK(M > 0 && M <= 64, "linear_bf16_small_m: M=%d out of range (1..64); use the wgmma GEMM", M);
   XB_CHECK(K % 32 == 0, "linear_bf16_small_m: K=%d must be a multiple of 32", K);
   XB_CHECK(x_stride % 8 == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0 &&
                (reinterpret_cast<uintptr_t>(w) & 15) == 0,

@@ -3,7 +3,7 @@
 // (xllm/core/kernels/cuda/batch_decode.cpp:26-86; planner
 //  xllm/core/layers/cuda/flashinfer_planinfo.cpp:249-337).
 //
-// Design (HBM-bound, B200):
+// Design (HBM-bound):
 //   grid = (kv splits, kv heads, batch).  One CTA streams one KV chunk of one
 //   (request, kv head): all GQA query heads of that kv head share the chunk, so
 //   every KV byte is read exactly once.  Per 16-token block a thread issues 16
@@ -613,7 +613,7 @@ extern "C" int xb_decode_plan(int64_t* plan8, int batch, int num_qo_heads, int n
            "decode_plan: bad heads %d/%d or batch %d", num_qo_heads, num_kv_heads, batch);
   XB_CHECK(head_dim == 64 || head_dim == 128, "decode_plan: head_dim %d unsupported (64|128)", head_dim);
   XB_CHECK(page_size > 0 && page_size < 65536 && max_pages_per_request > 0, "decode_plan: bad page geometry");
-  if (num_sms <= 0) num_sms = 148;
+  if (num_sms <= 0) num_sms = 132;
   const int group = num_qo_heads / num_kv_heads;
   const int head_tiles = (group + 15) / 16;
   const int64_t units = (int64_t)batch * num_kv_heads * head_tiles;
@@ -636,9 +636,9 @@ extern "C" int xb_decode_plan(int64_t* plan8, int batch, int num_qo_heads, int n
   // that use K = ceil(want / 16) clusters whose K results meet in the workspace (last-arriver merge).
   int64_t cluster = 1, parts = want;
   const char* envc = getenv("XB_DECODE_CLUSTER");  // 0 / 1: no clusters (every split is a workspace partial)
-  // Default 1 (no clusters).  Measured on B200 (tools/decode_sweep.py): the device co-schedules only 15 clusters of 8 / 9
-  // CTAs and 7 of 12 / 16 (GPCs are unevenly populated), so cluster geometries that fill the SMs run in two waves; the
-  // one that fits (16 CTAs x 1 cluster per kv head, 64 SMs) matches the cluster-less kernel.  The path stays available.
+  // Default 1 (no clusters): GPCs are unevenly populated, so the device co-schedules fewer large clusters than its SM count
+  // suggests and cluster geometries that fill the SMs can run in two waves (tools/decode_sweep.py measures it).  The path
+  // stays available.
   const int64_t cmax = envc ? atoi(envc) : 1;
   if (want > 1 && cmax > 1) {
     parts = (want + cmax - 1) / cmax;

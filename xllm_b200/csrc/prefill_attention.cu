@@ -1,21 +1,19 @@
-// Prefill / chunked-prefill attention on tcgen05 tensor cores with TMEM accumulators and TMA staging.
-// Replaces the FlashInfer fa2 (mma.sync) modules the reference dlopen()s on B200:
+// Prefill / chunked-prefill attention on wgmma tensor cores with TMA staging.
+// Replaces the FlashInfer fa2 (mma.sync) modules the reference dlopen()s:
 //   ragged_run  - xllm::kernel::cuda::batch_prefill          (kernels/cuda/batch_prefill.cpp:21-163): contiguous ragged q/k/v
 //   paged_run   - xllm::kernel::cuda::batch_chunked_prefill  (kernels/cuda/batch_chunked_prefill.cpp:26-92): ragged q over the
 //                 paged KV cache (chunked prefill with causal offset; also "decode on tensor cores", causal = false)
 //
-// One CTA per (q tile, kv head, request).  A q tile packs (token, head-of-the-GQA-group) pairs into the 128 MMA rows
+// One CTA per (q tile, kv head, request).  A q tile packs (token, head-of-the-GQA-group) pairs into 128 rows
 // (tokens_per_tile = 128 / group), so every K/V tile is fetched once per kv head for the whole group.
 //   warp 0      TMA producer: Q tile once (3-D tensor map token x head x d), then K and V tiles through 2-stage rings.
 //               Paged KV: one 2-D TMA per page fragment, the row coordinate comes from the page table.
-//   warp 1      MMA issuer (one elected lane):  S = Q K^T  (128 x 128 x d, both operands K-major, fp32 in TMEM, double
-//               buffered so S(j+1) is computed while softmax works on S(j));  O += P V  (P from smem K-major, V straight
-//               from its [kv, d] TMA tile as an MN-major operand - no transpose pass).
-//   warps 2..5  softmax / correction / epilogue, thread = row: tcgen05.ld the S row, base-2 online softmax
-//               (sm_scale*log2e folded), causal / length mask only on tiles that need it, P rounded to bf16 into the
-//               128B-swizzled smem tile (denominator summed from the ROUNDED P like the reference ladder), lazy
-//               O rescale with tcgen05.ld/st when the running max moved, final O / l -> bf16 -> global.
-// TMEM: S0 [0,128)  S1 [128,256)  O [256, 256+d).
+//   warps 4..11 two consumer warpgroups, warpgroup g owns rows 64 g .. 64 g + 63 of the tile:
+//               S = Q K^T (wgmma m64 x 128 x 16, both operands K-major in smem, fp32 in registers), base-2 online
+//               softmax (sm_scale*log2e folded; causal / length mask only on tiles that need it), P rounded to bf16
+//               (denominator summed from the ROUNDED P like the reference ladder) and kept in registers as the A operand
+//               of O += P V (V straight from its [kv, d] TMA tile as an MN-major operand - no transpose pass), final
+//               O / l -> bf16 -> global.
 #include <type_traits>
 
 #include "tc_common.cuh"
@@ -42,16 +40,10 @@ struct PrefillParams {
   float* part_o;                   // [kv_splits][total_q][Hq][D]
   float* part_lse;                 // [kv_splits][total_q][Hq]
   int64_t total_q;
-  // ping-pong kernel: a row adopts a new running maximum (and rescales O) only when it grew by more than rescale_tau
-  // (base-2 units); below that P = 2^(s - m_stale) <= 2^tau stays exact enough in bf16 / fp32 and the O correction
-  // (TMEM load + multiply + store of the whole accumulator row) is skipped.  0 = the reference ladder (always adopt).
-  float rescale_tau;
-  int qk_first;      // ping-pong kernel: issue QK_x(j+1) before PV_x(j) (S_x(j+1) is ready one MMA earlier)
-  int spin_mma;      // ping-pong kernel: the MMA issuer polls its barriers without the suspend hint
 };
 
-constexpr int kQT = 128;   // MMA rows
 constexpr int kKT = 128;   // kv tile
+constexpr int kPrefillThreads = 384;
 
 template <int kD>
 struct PrefillCfg {
@@ -59,13 +51,11 @@ struct PrefillCfg {
   static constexpr int kSub = 128 * 128;                           // one [128 rows x 64 elems] swizzled sub-tile
   static constexpr int kQBytes = kHalves * kSub;
   static constexpr int kKVBytes = kHalves * kSub;                  // K tile or V tile
-  static constexpr int kPBytes = 2 * kSub;                         // P [128 x 128 kv]
-  static constexpr int kSmemBytes = kQBytes + 4 * kKVBytes + kPBytes + 1024 + 256;
-  static constexpr int kTmemCols = 512;
+  static constexpr int kSmemBytes = kQBytes + 4 * kKVBytes + 1024 + 256;
 };
 
 template <int kD>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(kPrefillThreads, 1)
 prefill_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
                          const __grid_constant__ CUtensorMap tmap_v, const PrefillParams p) {
   using Cfg = PrefillCfg<kD>;
@@ -74,18 +64,12 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gri
   uint8_t* q_s = smem;
   uint8_t* k_s = q_s + Cfg::kQBytes;                // [2][kKVBytes]
   uint8_t* v_s = k_s + 2 * Cfg::kKVBytes;           // [2][kKVBytes]
-  uint8_t* p_s = v_s + 2 * Cfg::kKVBytes;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(p_s + Cfg::kPBytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(v_s + 2 * Cfg::kKVBytes);
   uint64_t* q_full = bars;            // 1
   uint64_t* k_full = bars + 1;        // 2
   uint64_t* k_empty = bars + 3;       // 2
   uint64_t* v_full = bars + 5;        // 2
   uint64_t* v_empty = bars + 7;       // 2
-  uint64_t* s_full = bars + 9;        // 2
-  uint64_t* s_empty = bars + 11;      // 2
-  uint64_t* p_full = bars + 13;       // 1
-  uint64_t* pv_done = bars + 14;      // 1
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(bars + 16);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int b = blockIdx.z / p.kv_splits, split = blockIdx.z - b * p.kv_splits, kvh = blockIdx.y;
@@ -95,14 +79,10 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gri
     mbar_init(q_full, 1);
     for (int i = 0; i < 2; ++i) {
       mbar_init(k_full + i, 1);
-      mbar_init(k_empty + i, 1);
+      mbar_init(k_empty + i, 8);      // one arrive per consumer warp
       mbar_init(v_full + i, 1);
-      mbar_init(v_empty + i, 1);
-      mbar_init(s_full + i, 1);
-      mbar_init(s_empty + i, 4);
+      mbar_init(v_empty + i, 8);
     }
-    mbar_init(p_full, 4);
-    mbar_init(pv_done, 1);
     fence_barrier_init();
   }
   if (warp == 0 && lane == 0) {
@@ -110,11 +90,7 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gri
     tma_prefetch_desc(&tmap_k);
     tma_prefetch_desc(&tmap_v);
   }
-  if (warp == 1) tmem_alloc(tmem_base_smem, Cfg::kTmemCols);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_base_smem;
   pdl_launch_dependents();
   pdl_wait();
 
@@ -177,573 +153,139 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gri
         }
       }
     }
-  } else if (warp == 1) {
-    // ============================== MMA issuer ==============================
-    constexpr uint32_t idesc_qk = umma_idesc(1, 1, kQT, kKT);
-    constexpr uint32_t idesc_pv = umma_idesc(1, 1, kQT, kD, 0, 1);     // B = V is MN-major
-    const uint32_t s_tmem[2] = {tmem_base, tmem_base + 128};
-    const uint32_t o_tmem = tmem_base + 256;
-    auto issue_qk = [&](int j) {
-      const int st = j & 1;
-      mbar_wait(k_full + st, (j >> 1) & 1);
-      mbar_wait(s_empty + st, ((j >> 1) & 1) ^ 1);
-      tc_fence_after_sync();
-      if (lane == 0) {
-        const uint32_t qa = smem_u32(q_s), ka = smem_u32(k_s + st * Cfg::kKVBytes);
+  } else if (warp >= 4) {
+    // ============================== consumers: S, softmax, O ==============================
+    // thread (warp w of warpgroup g, lane l) holds rows rr[h] = 64 g + 16 w + l / 4 + 8 h (h = 0, 1) and columns
+    // 8 j + 2 (l % 4) + e of every accumulator (tc_common.cuh fragment layout)
+    const int wg = (warp - 4) >> 2, wq = warp & 3;
+    const int cq = 2 * (lane & 3);
+    int my_lim[2];
+    bool row_valid[2];
+    int q_idx[2], head_local[2];
 #pragma unroll
-        for (int s = 0; s < kD / 16; ++s) {
-          const uint32_t off = (s >> 2) * Cfg::kSub + (s & 3) * 32;
-          umma_f16(s_tmem[st], umma_desc_sw128(qa + off), umma_desc_sw128(ka + off), idesc_qk, s != 0);
-        }
-        umma_commit(k_empty + st);
-        umma_commit(s_full + st);
-      }
-      __syncwarp();
-    };
-    if (n_tiles > 0) {
-      mbar_wait(q_full, 0);
-      issue_qk(0);
-      for (int j = 0; j < n_tiles; ++j) {
-        if (j + 1 < n_tiles) issue_qk(j + 1);
-        const int st = j & 1;
-        mbar_wait(v_full + st, (j >> 1) & 1);
-        mbar_wait(p_full, j & 1);
-        tc_fence_after_sync();
-        if (lane == 0) {
-          const uint32_t pa = smem_u32(p_s), va = smem_u32(v_s + st * Cfg::kKVBytes);
-#pragma unroll
-          for (int s = 0; s < kKT / 16; ++s) {
-            const uint64_t da = umma_desc_sw128(pa + (s >> 2) * Cfg::kSub + (s & 3) * 32);
-            const uint64_t db = umma_desc_sw128_mn(va + s * 2048, Cfg::kSub, 1024);
-            umma_f16(o_tmem, da, db, idesc_pv, (j | s) != 0);
-          }
-          umma_commit(v_empty + st);
-          umma_commit(pv_done);
-        }
-        __syncwarp();
-      }
+    for (int h = 0; h < 2; ++h) {
+      const int r = wg * 64 + wq * 16 + (lane >> 2) + 8 * h;
+      const int tok_local = r / p.group;
+      head_local[h] = r - tok_local * p.group;
+      q_idx[h] = tq0 + tok_local;
+      row_valid[h] = live && r < rows_used && q_idx[h] < qo_len;
+      my_lim[h] = p.causal ? min(kv_len, q_idx[h] + kv_off + 1) : kv_len;        // #visible keys of the row
     }
-  } else {
-    // ============================== softmax / correction / epilogue ==============================
-    const int qd = warp & 3;
-    const int r = qd * 32 + lane;                       // my row of the tile = my TMEM lane
-    const uint32_t lane_addr = (uint32_t)(qd * 32) << 16;
-    const int tok_local = r / p.group, head_local = r - tok_local * p.group;
-    const int q_idx = tq0 + tok_local;
-    const bool row_valid = live && r < rows_used && q_idx < qo_len;
-    const int my_lim = p.causal ? min(kv_len, q_idx + kv_off + 1) : kv_len;       // #visible keys of my row
     const int lim_first = p.causal ? min(kv_len, tq0 + kv_off + 1) : kv_len;      // smallest limit in the tile
-    float m_run = -INFINITY, l_run = 0.f;
-    const uint32_t o_tmem = tmem_base + 256 + lane_addr;
+    float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};            // l_run: this thread's columns only
+    float o[kD / 2];
+#pragma unroll
+    for (int i = 0; i < kD / 2; ++i) o[i] = 0.f;
+    float s[kKT / 2];
+    if (n_tiles > 0) mbar_wait(q_full, 0);
 
     for (int j = 0; j < n_tiles; ++j) {
-      const int sb = j & 1;
-      const uint32_t s_tmem = tmem_base + sb * 128 + lane_addr;
-      mbar_wait(s_full + sb, (j >> 1) & 1);
-      tc_fence_after_sync();
+      const int st = j & 1;
+      const uint32_t par = (j >> 1) & 1;
+      // ---- S = Q K^T ----
+      mbar_wait(k_full + st, par);
+      {
+        const uint32_t qa = smem_u32(q_s) + wg * 64 * 128, ka = smem_u32(k_s + st * Cfg::kKVBytes);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kD / 16; ++k) {
+          const uint32_t off = (k >> 2) * Cfg::kSub + (k & 3) * 32;
+          wgmma_bf16<kKT>(s, gmma_desc_sw128(qa + off), gmma_desc_sw128(ka + off), k > 0 ? 1u : 0u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_operands(s);
+      }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(k_empty + st);
       const bool need_mask = (j0 + j + 1) * kKT > lim_first;
-      const int col_lim = my_lim - (j0 + j) * kKT;      // columns >= col_lim are masked
-      // ---- pass 1: row max ----
-      float mx = -INFINITY;
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(s_tmem + c * 32, v);
-        tmem_ld_wait();
-        if (need_mask) {
+      // ---- online softmax (the four lanes of a row reduce with shuffles) ----
+      float alpha[2], m_safe[2];
 #pragma unroll
-          for (int i = 0; i < 32; ++i) mx = fmaxf(mx, (c * 32 + i) < col_lim ? __uint_as_float(v[i]) : -INFINITY);
-        } else {
+      for (int h = 0; h < 2; ++h) {
+        const int col_lim = my_lim[h] - (j0 + j) * kKT;      // columns >= col_lim are masked
+        float mx = -INFINITY;
 #pragma unroll
-          for (int i = 0; i < 32; ++i) mx = fmaxf(mx, __uint_as_float(v[i]));
-        }
-      }
-      const float m_new = fmaxf(m_run, mx * p.scale_log2);
-      const float m_safe = m_new == -INFINITY ? 0.f : m_new;
-      const float alpha = fast_exp2(m_run - m_safe);
-      // ---- P smem / O are free once PV(j-1) has completed ----
-      if (j > 0) {
-        mbar_wait(pv_done, (j - 1) & 1);
-        tc_fence_after_sync();
-        if (__any_sync(0xffffffffu, alpha < 1.0f)) {     // lazy correction: only when some row's max moved
-#pragma unroll 1
-          for (int c = 0; c < kD / 32; ++c) {
-            uint32_t v[32];
-            tmem_ld_32x32b_x32(o_tmem + c * 32, v);
-            tmem_ld_wait();
+        for (int jj = 0; jj < kKT / 8; ++jj)
 #pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * alpha);
-            tmem_st_32x32b_x32(o_tmem + c * 32, v);
+          for (int e = 0; e < 2; ++e) {
+            const float v = s[4 * jj + 2 * h + e];
+            mx = fmaxf(mx, (!need_mask || 8 * jj + cq + e < col_lim) ? v : -INFINITY);
           }
-          tmem_st_wait();
-        }
-      }
-      // ---- pass 2: P = exp2(s*scale - m), rounded to bf16, into the swizzled [128 x 128] K-major tile ----
-      float psum = 0.f;
-#pragma unroll 1
-      for (int c = 0; c < 4; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32b_x32(s_tmem + c * 32, v);
-        tmem_ld_wait();
-        uint32_t pk[16];
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+        const float m_new = fmaxf(m_run[h], mx * p.scale_log2);
+        m_safe[h] = m_new == -INFINITY ? 0.f : m_new;
+        alpha[h] = fast_exp2(m_run[h] - m_safe[h]);
+        m_run[h] = m_new;
+        float psum = 0.f;
 #pragma unroll
-        for (int i = 0; i < 32; i += 2) {
-          float p0 = fast_exp2(__uint_as_float(v[i]) * p.scale_log2 - m_safe);
-          float p1 = fast_exp2(__uint_as_float(v[i + 1]) * p.scale_log2 - m_safe);
+        for (int jj = 0; jj < kKT / 8; ++jj) {
+          const int i0 = 4 * jj + 2 * h;
+          float p0 = fast_exp2(s[i0] * p.scale_log2 - m_safe[h]);
+          float p1 = fast_exp2(s[i0 + 1] * p.scale_log2 - m_safe[h]);
           if (need_mask) {
-            if (c * 32 + i >= col_lim) p0 = 0.f;
-            if (c * 32 + i + 1 >= col_lim) p1 = 0.f;
+            if (8 * jj + cq >= col_lim) p0 = 0.f;
+            if (8 * jj + cq + 1 >= col_lim) p1 = 0.f;
           }
           const uint32_t pp = pack_bf16x2(p0, p1);
-          pk[i >> 1] = pp;
-          psum += bf16lo(pp) + bf16hi(pp);              // denominator from the ROUNDED P (reference ladder)
+          s[i0] = __uint_as_float(pp);                 // the bf16 pair, as the A fragment of P V below
+          psum += bf16lo(pp) + bf16hi(pp);             // denominator from the ROUNDED P (reference ladder)
         }
-        // row r, columns [32c, 32c+32): sub-tile (c >> 1), 16-byte chunks ((c & 1) * 4 + i) ^ (r & 7)
-        uint8_t* rowp = p_s + (c >> 1) * Cfg::kSub + r * 128;
+        l_run[h] = l_run[h] * alpha[h] + psum;
+      }
 #pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const int chunk = ((c & 1) * 4 + i) ^ (r & 7);
-          *reinterpret_cast<uint4*>(rowp + (chunk << 4)) = make_uint4(pk[4 * i], pk[4 * i + 1], pk[4 * i + 2], pk[4 * i + 3]);
+      for (int jj = 0; jj < kD / 8; ++jj)
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          o[4 * jj + 2 * h] *= alpha[h];
+          o[4 * jj + 2 * h + 1] *= alpha[h];
         }
+      // ---- O += P V: A fragment of k step kk = S columns 16 kk .. 16 kk + 15 (rows h = 0, 1; column halves 0, 1) ----
+      mbar_wait(v_full + st, par);
+      {
+        const uint32_t va = smem_u32(v_s + st * Cfg::kKVBytes);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < kKT / 16; ++kk) {
+          const uint32_t a[4] = {__float_as_uint(s[8 * kk + 0]), __float_as_uint(s[8 * kk + 2]), __float_as_uint(s[8 * kk + 4]),
+                                 __float_as_uint(s[8 * kk + 6])};
+          wgmma_bf16_rs_tb<kD>(o, a, gmma_desc_sw128_mn(va + kk * 2048, Cfg::kSub, 1024), 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        wgmma_fence_operands(o);
       }
-      l_run = l_run * alpha + psum;
-      m_run = m_new;
-      tc_fence_before_sync();          // my TMEM reads of S (and O stores) are ordered before the arrives below
-      fence_proxy_async_smem();        // P stores -> visible to the tensor core
       __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(s_empty + sb);
-        mbar_arrive(p_full);
-      }
+      if (lane == 0) mbar_arrive(v_empty + st);
     }
     // ---- epilogue: O / l -> bf16 -> global ----
-    if (n_tiles > 0) {
-      mbar_wait(pv_done, (n_tiles - 1) & 1);
-      tc_fence_after_sync();
-    }
-    const float inv = l_run > 0.f ? 1.0f / l_run : 0.f;
-    __nv_bfloat16* dst = nullptr;
-    float* pdst = nullptr;
-    if (row_valid) {
-      const int64_t tq = q0 + q_idx;
-      const int head = kvh * p.group + head_local;
-      const float lse2 = l_run > 0.f ? m_run + log2f(l_run) : -INFINITY;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float l = l_run[h];
+      l += __shfl_xor_sync(0xffffffffu, l, 1);
+      l += __shfl_xor_sync(0xffffffffu, l, 2);
+      if (!row_valid[h]) continue;
+      const float inv = l > 0.f ? 1.0f / l : 0.f;
+      const int64_t tq = q0 + q_idx[h];
+      const int head = kvh * p.group + head_local[h];
+      const float lse2 = l > 0.f ? m_run[h] + log2f(l) : -INFINITY;
       if (p.kv_splits == 1) {
-        dst = p.o + tq * p.o_stride_n + (int64_t)head * p.o_stride_h;
-        if (p.lse) p.lse[tq * p.num_qo_heads + head] = lse2;
+        __nv_bfloat16* dst = p.o + tq * p.o_stride_n + (int64_t)head * p.o_stride_h;
+        if (p.lse && (lane & 3) == 0) p.lse[tq * p.num_qo_heads + head] = lse2;
+#pragma unroll
+        for (int jj = 0; jj < kD / 8; ++jj)
+          *reinterpret_cast<uint32_t*>(dst + 8 * jj + cq) = pack_bf16x2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
       } else {
         const int64_t slot = ((int64_t)split * p.total_q + tq) * p.num_qo_heads + head;
-        pdst = p.part_o + slot * kD;
-        p.part_lse[slot] = lse2;
-      }
-    }
-#pragma unroll 1
-    for (int c = 0; c < kD / 32; ++c) {
-      uint32_t v[32];
-      if (n_tiles > 0) {
-        tmem_ld_32x32b_x32(o_tmem + c * 32, v);
-        tmem_ld_wait();
-      } else {
+        float* pdst = p.part_o + slot * kD;
+        if ((lane & 3) == 0) p.part_lse[slot] = lse2;
 #pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = 0;
-      }
-      if (dst) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          uint4 o;
-          o.x = pack_bf16x2(__uint_as_float(v[8 * i + 0]) * inv, __uint_as_float(v[8 * i + 1]) * inv);
-          o.y = pack_bf16x2(__uint_as_float(v[8 * i + 2]) * inv, __uint_as_float(v[8 * i + 3]) * inv);
-          o.z = pack_bf16x2(__uint_as_float(v[8 * i + 4]) * inv, __uint_as_float(v[8 * i + 5]) * inv);
-          o.w = pack_bf16x2(__uint_as_float(v[8 * i + 6]) * inv, __uint_as_float(v[8 * i + 7]) * inv);
-          *reinterpret_cast<uint4*>(dst + c * 32 + i * 8) = o;
-        }
-      } else if (pdst) {
-#pragma unroll
-        for (int i = 0; i < 8; ++i)
-          *reinterpret_cast<float4*>(pdst + c * 32 + i * 4) =
-              make_float4(__uint_as_float(v[4 * i]) * inv, __uint_as_float(v[4 * i + 1]) * inv,
-                          __uint_as_float(v[4 * i + 2]) * inv, __uint_as_float(v[4 * i + 3]) * inv);
+        for (int jj = 0; jj < kD / 8; ++jj)
+          *reinterpret_cast<float2*>(pdst + 8 * jj + cq) = make_float2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
       }
     }
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, Cfg::kTmemCols);
-}
-
-// ------------------------------------------------------------------------------------------------------------------
-// Ping-pong variant (kv_splits == 1): one CTA owns TWO adjacent q tiles (A, B) of a (request, kv head) and two softmax
-// warpgroups, so the tensor core always has the other tile's MMAs to run while one tile is in its softmax:
-//   tensor-core order per kv tile j:  PV_A(j)  QK_A(j+1)  PV_B(j)  QK_B(j+1)
-//   warpgroup A works on S_A(j) while PV_B(j-1) / QK_B(j) execute, warpgroup B on S_B(j) while PV_A(j) / QK_A(j+1) do.
-// Both tiles read the same K / V tiles (fetched once per pair).  The S accumulator of a tile is single-buffered (the
-// other tile is the second buffer); P goes through a per-tile swizzled smem tile; tcgen05.ld of the S row is software
-// pipelined against the exponentials of the previous 32 columns.
-//   warp 0 TMA producer | warp 1 MMA issuer | warps 2..5 softmax A | warps 6..9 softmax B  (TMEM lane quarter = warp % 4)
-// TMEM: S_A [0,128)  S_B [128,256)  O_A [256,256+d)  O_B [384,384+d).
-// smem (d = 128): Q_A Q_B 64 KB | K x2 64 KB | V x1 32 KB | P_A P_B 64 KB = 224 KB.
-template <int kD>
-struct Prefill2Cfg {
-  static constexpr int kHalves = kD / 64;
-  static constexpr int kSub = 128 * 128;
-  static constexpr int kQBytes = kHalves * kSub;
-  static constexpr int kKVBytes = kHalves * kSub;
-  static constexpr int kPBytes = 2 * kSub;
-  static constexpr int kVStages = kD == 128 ? 1 : 2;
-  static constexpr int kSmemBytes = 2 * kQBytes + (2 + kVStages) * kKVBytes + 2 * kPBytes + 1024 + 256;
-  static constexpr int kTmemCols = 512;
-  static constexpr int kThreads = 320;
-};
-
-template <int kD>
-__global__ void __launch_bounds__(Prefill2Cfg<kD>::kThreads, 1)
-prefill_attention2_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                          const __grid_constant__ CUtensorMap tmap_v, const PrefillParams p) {
-  using Cfg = Prefill2Cfg<kD>;
-  constexpr int kVS = Cfg::kVStages;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* q_s = smem;                               // [2][kQBytes]   tile A, tile B
-  uint8_t* k_s = q_s + 2 * Cfg::kQBytes;             // [2][kKVBytes]
-  uint8_t* v_s = k_s + 2 * Cfg::kKVBytes;            // [kVS][kKVBytes]
-  uint8_t* p_s = v_s + kVS * Cfg::kKVBytes;          // [2][kPBytes]   tile A, tile B
-  uint64_t* bars = reinterpret_cast<uint64_t*>(p_s + 2 * Cfg::kPBytes);
-  uint64_t* q_full = bars;            // [2] per tile
-  uint64_t* k_full = bars + 2;        // [2] per stage
-  uint64_t* k_empty = bars + 4;       // [2]
-  uint64_t* v_full = bars + 6;        // [2] per stage (kVS used)
-  uint64_t* v_empty = bars + 8;       // [2]
-  uint64_t* s_full = bars + 10;       // [2] per tile
-  uint64_t* p_full = bars + 12;       // [2] per tile
-  uint64_t* pv_done = bars + 14;      // [2] per tile
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(bars + 16);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int b = blockIdx.z, kvh = blockIdx.y;
-  const int pair = gridDim.x - 1 - blockIdx.x;        // heavy (late, causal) pairs first
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(q_full + i, 1);
-      mbar_init(k_full + i, 1);
-      mbar_init(k_empty + i, 1);
-      mbar_init(v_full + i, 1);
-      mbar_init(v_empty + i, 1);
-      mbar_init(s_full + i, 1);
-      mbar_init(p_full + i, 4);
-      mbar_init(pv_done + i, 1);
-    }
-    fence_barrier_init();
-  }
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmap_q);
-    tma_prefetch_desc(&tmap_k);
-    tma_prefetch_desc(&tmap_v);
-  }
-  if (warp == 1) tmem_alloc(tmem_base_smem, Cfg::kTmemCols);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_base_smem;
-  pdl_launch_dependents();
-  pdl_wait();
-
-  // ---- work item geometry (uniform across the CTA) ------------------------------------------------------------
-  const int q0 = __ldg(p.qo_indptr + b);
-  const int qo_len = __ldg(p.qo_indptr + b + 1) - q0;
-  int kv_len, kv_base = 0, indptr0 = 0, n_pages = 0;
-  if (p.paged) {
-    indptr0 = __ldg(p.kv_indptr + b);
-    n_pages = __ldg(p.kv_indptr + b + 1) - indptr0;
-    kv_len = n_pages > 0 ? (n_pages - 1) * p.page_size + __ldg(p.kv_last_page_len + b) : 0;
-  } else {
-    kv_base = __ldg(p.kv_indptr + b);
-    kv_len = __ldg(p.kv_indptr + b + 1) - kv_base;
-  }
-  const int kv_off = kv_len - qo_len;                  // causal offset of chunked prefill (prefill.cuh:1017 semantics)
-  const int rows_used = p.tokens_per_tile * p.group;
-  int tq0x[2], ntx[2];
-  bool livex[2];
-#pragma unroll
-  for (int x = 0; x < 2; ++x) {
-    tq0x[x] = (2 * pair + x) * p.tokens_per_tile;       // first q token of tile x (request-local)
-    livex[x] = tq0x[x] < qo_len;
-    const int tq_last = min(qo_len, tq0x[x] + p.tokens_per_tile) - 1;
-    int kv_limit = p.causal ? min(kv_len, tq_last + kv_off + 1) : kv_len;
-    if (kv_limit < 0) kv_limit = 0;
-    ntx[x] = livex[x] ? (kv_limit + kKT - 1) / kKT : 0;
-  }
-  const int n_max = max(ntx[0], ntx[1]);
-
-  if (warp == 0) {
-    // ============================== TMA producer ==============================
-    if (lane == 0 && n_max > 0) {
-#pragma unroll
-      for (int x = 0; x < 2; ++x) {
-        if (ntx[x] > 0) {
-          mbar_expect_tx(q_full + x, rows_used * kD * 2);
-#pragma unroll
-          for (int h = 0; h < Cfg::kHalves; ++h)
-            tma_load_3d(q_s + x * Cfg::kQBytes + h * Cfg::kSub, &tmap_q, q_full + x, h * 64, kvh * p.group, q0 + tq0x[x]);
-        }
-      }
-      const int loads = kKT / p.box_rows;
-      auto load_tile = [&](int j, int is_v) {
-        const int st = is_v ? (j % kVS) : (j & 1);
-        const int use = is_v ? (j / kVS) : (j >> 1);        // how many times this stage has been filled before
-        uint64_t* full = is_v ? v_full + st : k_full + st;
-        mbar_wait(is_v ? v_empty + st : k_empty + st, (use & 1) ^ 1);
-        mbar_expect_tx(full, kKT * kD * 2);
-        uint8_t* dst = (is_v ? v_s : k_s) + st * Cfg::kKVBytes;
-        const CUtensorMap* map = is_v ? &tmap_v : &tmap_k;
-        for (int i = 0; i < loads; ++i) {
-          const int t0 = j * kKT + i * p.box_rows;
-          int row;
-          if (p.paged) {
-            int pg = t0 / p.page_size;
-            if (pg >= n_pages) pg = n_pages - 1;    // beyond the request: masked anyway, keep the address valid
-            row = __ldg(p.kv_indices + indptr0 + pg) * p.page_size + (t0 % p.page_size);
-          } else {
-            row = kv_base + t0;
-          }
-#pragma unroll
-          for (int h = 0; h < Cfg::kHalves; ++h)
-            tma_load_2d(dst + h * Cfg::kSub + i * p.box_rows * 128, map, full, kvh * kD + h * 64, row);
-        }
-      };
-      load_tile(0, 0);
-      for (int j = 0; j < n_max; ++j) {
-        if (j + 1 < n_max) load_tile(j + 1, 0);     // K(j+1) is wanted right after PV_A(j)
-        load_tile(j, 1);
-      }
-    }
-  } else if (warp == 1) {
-    // ============================== MMA issuer ==============================
-    constexpr uint32_t idesc_qk = umma_idesc(1, 1, kQT, kKT);
-    constexpr uint32_t idesc_pv = umma_idesc(1, 1, kQT, kD, 0, 1);     // B = V is MN-major
-    auto issue_qk = [&](int x, int j) {                 // S_x = Q_x K(j)^T
-      if (lane == 0) {
-        const uint32_t qa = smem_u32(q_s + x * Cfg::kQBytes), ka = smem_u32(k_s + (j & 1) * Cfg::kKVBytes);
-#pragma unroll
-        for (int s = 0; s < kD / 16; ++s) {
-          const uint32_t off = (s >> 2) * Cfg::kSub + (s & 3) * 32;
-          umma_f16(tmem_base + x * 128, umma_desc_sw128(qa + off), umma_desc_sw128(ka + off), idesc_qk, s != 0);
-        }
-        umma_commit(s_full + x);
-      }
-      __syncwarp();
-    };
-    auto issue_pv = [&](int x, int j) {                 // O_x += P_x V(j)
-      if (lane == 0) {
-        const uint32_t pa = smem_u32(p_s + x * Cfg::kPBytes), va = smem_u32(v_s + (j % kVS) * Cfg::kKVBytes);
-#pragma unroll
-        for (int s = 0; s < kKT / 16; ++s) {
-          const uint64_t da = umma_desc_sw128(pa + (s >> 2) * Cfg::kSub + (s & 3) * 32);
-          const uint64_t db = umma_desc_sw128_mn(va + s * 2048, Cfg::kSub, 1024);
-          umma_f16(tmem_base + 256 + x * 128, da, db, idesc_pv, (j | s) != 0);
-        }
-        umma_commit(pv_done + x);
-      }
-      __syncwarp();
-    };
-    if (n_max > 0) {
-      mbar_wait(k_full + 0, 0);
-#pragma unroll
-      for (int x = 0; x < 2; ++x) {
-        if (ntx[x] > 0) {
-          mbar_wait(q_full + x, 0);
-          tc_fence_after_sync();
-          issue_qk(x, 0);
-        }
-      }
-      if (lane == 0) umma_commit(k_empty + 0);
-      __syncwarp();
-      for (int j = 0; j < n_max; ++j) {
-        const bool more = j + 1 < n_max;
-        bool k_ready = false, v_ready = false;
-#pragma unroll
-        for (int x = 0; x < 2; ++x) {
-          const bool do_pv = j < ntx[x], do_qk = j + 1 < ntx[x];
-          if (do_pv) {
-            if (p.spin_mma) mbar_wait_spin(p_full + x, j & 1);
-            else mbar_wait(p_full + x, j & 1);               // P_x(j) written; S_x(j) fully read
-          }
-          if (do_qk && !k_ready) {
-            mbar_wait(k_full + ((j + 1) & 1), ((j + 1) >> 1) & 1);
-            k_ready = true;
-          }
-          if (do_pv && !v_ready) {
-            mbar_wait(v_full + (j % kVS), (j / kVS) & 1);
-            v_ready = true;
-          }
-          tc_fence_after_sync();
-          if (p.qk_first) {
-            if (do_qk) issue_qk(x, j + 1);
-            if (do_pv) issue_pv(x, j);
-          } else {
-            if (do_pv) issue_pv(x, j);
-            if (do_qk) issue_qk(x, j + 1);
-          }
-        }
-        if (lane == 0) {
-          umma_commit(v_empty + (j % kVS));             // after the last PV that reads V(j)
-          if (more) umma_commit(k_empty + ((j + 1) & 1));   // after the last QK that reads K(j+1)
-        }
-        __syncwarp();
-      }
-    }
-  } else {
-    // ============================== softmax / correction / epilogue: warpgroup x owns tile x ==============================
-    const int x = (warp - 2) >> 2;                      // 0: tile A (warps 2..5), 1: tile B (warps 6..9)
-    const int qd = warp & 3;                            // TMEM lane quarter this warp may access
-    const int r = qd * 32 + lane;                       // my row of the tile = my TMEM lane
-    const uint32_t lane_addr = (uint32_t)(qd * 32) << 16;
-    const int tq0 = tq0x[x], n_tiles = ntx[x];
-    const bool live = livex[x];
-    const int tok_local = r / p.group, head_local = r - tok_local * p.group;
-    const int q_idx = tq0 + tok_local;
-    const bool row_valid = live && r < rows_used && q_idx < qo_len;
-    const int my_lim = p.causal ? min(kv_len, q_idx + kv_off + 1) : kv_len;       // #visible keys of my row
-    const int lim_first = p.causal ? min(kv_len, tq0 + kv_off + 1) : kv_len;      // smallest limit in the tile
-    float m_run = -INFINITY, l_run = 0.f;
-    const uint32_t s_tmem = tmem_base + x * 128 + lane_addr;
-    const uint32_t o_tmem = tmem_base + 256 + x * 128 + lane_addr;
-    uint8_t* my_p = p_s + x * Cfg::kPBytes;
-    const float sc = p.scale_log2;
-
-    for (int j = 0; j < n_tiles; ++j) {
-      mbar_wait(s_full + x, j & 1);
-      tc_fence_after_sync();
-      const bool need_mask = (j + 1) * kKT > lim_first;
-      const int col_lim = my_lim - j * kKT;             // columns >= col_lim are masked
-      // ---- pass 1: row max; the load of the next 32 columns is in flight while these are reduced.  The masked and the
-      // unmasked sweep are two separate code paths (a per-element `if (need_mask)` is if-converted into ISETP + FSEL on
-      // EVERY tile: 2.3 of 12 instructions per element of the first version) ----
-      float mx = -INFINITY;
-      auto pass1 = [&](auto masked) {
-        constexpr bool kMask = decltype(masked)::value;
-        uint32_t va[32], vb[32];
-        tmem_ld_32x32b_x32(s_tmem, va);
-        tmem_ld_wait(va);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint32_t (&cur)[32] = (c & 1) ? vb : va;
-          uint32_t (&nxt)[32] = (c & 1) ? va : vb;
-          if (c < 3) tmem_ld_32x32b_x32(s_tmem + (c + 1) * 32, nxt);
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            if (kMask) mx = fmaxf(mx, (c * 32 + i) < col_lim ? __uint_as_float(cur[i]) : -INFINITY);
-            else mx = fmaxf(mx, __uint_as_float(cur[i]));
-          }
-          if (c < 3) tmem_ld_wait(nxt);
-        }
-      };
-      if (need_mask) pass1(std::true_type{});
-      else pass1(std::false_type{});
-      const float m_cand = fmaxf(m_run, mx * sc);
-      const float m_new = (m_cand - m_run > p.rescale_tau) ? m_cand : m_run;    // (-inf start: inf > tau adopts)
-      const float m_safe = m_new == -INFINITY ? 0.f : m_new;
-      const float alpha = fast_exp2(m_run - m_safe);
-      // ---- P_x smem / O_x are free once PV_x(j-1) has completed ----
-      if (j > 0) {
-        mbar_wait(pv_done + x, (j - 1) & 1);
-        tc_fence_after_sync();
-        if (__any_sync(0xffffffffu, alpha < 1.0f)) {     // lazy correction: only when some row's max moved
-#pragma unroll 1
-          for (int c = 0; c < kD / 32; ++c) {
-            uint32_t v[32];
-            tmem_ld_32x32b_x32(o_tmem + c * 32, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; ++i) v[i] = __float_as_uint(__uint_as_float(v[i]) * alpha);
-            tmem_st_32x32b_x32(o_tmem + c * 32, v);
-          }
-          tmem_st_wait();
-        }
-      }
-      // ---- pass 2: P = exp2(s*scale - m), rounded to bf16, into the swizzled [128 x 128] K-major tile ----
-      float psum = 0.f;
-      auto pass2 = [&](auto masked) {
-        constexpr bool kMask = decltype(masked)::value;
-        uint32_t va[32], vb[32];
-        tmem_ld_32x32b_x32(s_tmem, va);
-        tmem_ld_wait(va);
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint32_t (&cur)[32] = (c & 1) ? vb : va;
-          uint32_t (&nxt)[32] = (c & 1) ? va : vb;
-          if (c < 3) tmem_ld_32x32b_x32(s_tmem + (c + 1) * 32, nxt);
-          uint32_t pk[16];
-#pragma unroll
-          for (int i = 0; i < 32; i += 2) {
-            float p0 = fast_exp2(fmaf(__uint_as_float(cur[i]), sc, -m_safe));
-            float p1 = fast_exp2(fmaf(__uint_as_float(cur[i + 1]), sc, -m_safe));
-            if (kMask) {
-              if (c * 32 + i >= col_lim) p0 = 0.f;
-              if (c * 32 + i + 1 >= col_lim) p1 = 0.f;
-            }
-            const uint32_t pp = pack_bf16x2(p0, p1);
-            pk[i >> 1] = pp;
-            psum += bf16lo(pp) + bf16hi(pp);              // denominator from the ROUNDED P (reference ladder)
-          }
-          // row r, columns [32c, 32c+32): sub-tile (c >> 1), 16-byte chunks ((c & 1) * 4 + i) ^ (r & 7)
-          uint8_t* rowp = my_p + (c >> 1) * Cfg::kSub + r * 128;
-#pragma unroll
-          for (int i = 0; i < 4; ++i) {
-            const int chunk = ((c & 1) * 4 + i) ^ (r & 7);
-            *reinterpret_cast<uint4*>(rowp + (chunk << 4)) = make_uint4(pk[4 * i], pk[4 * i + 1], pk[4 * i + 2], pk[4 * i + 3]);
-          }
-          if (c < 3) tmem_ld_wait(nxt);
-        }
-      };
-      if (need_mask) pass2(std::true_type{});
-      else pass2(std::false_type{});
-      l_run = l_run * alpha + psum;
-      m_run = m_new;
-      tc_fence_before_sync();          // my TMEM reads of S (and O stores) are ordered before the arrive below
-      fence_proxy_async_smem();        // P stores -> visible to the tensor core
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full + x);
-    }
-    // ---- epilogue: O / l -> bf16 -> global ----
-    if (n_tiles > 0) {
-      mbar_wait(pv_done + x, (n_tiles - 1) & 1);
-      tc_fence_after_sync();
-    }
-    const float inv = l_run > 0.f ? 1.0f / l_run : 0.f;
-    __nv_bfloat16* dst = nullptr;
-    if (row_valid) {
-      const int64_t tq = q0 + q_idx;
-      const int head = kvh * p.group + head_local;
-      dst = p.o + tq * p.o_stride_n + (int64_t)head * p.o_stride_h;
-      if (p.lse) p.lse[tq * p.num_qo_heads + head] = l_run > 0.f ? m_run + log2f(l_run) : -INFINITY;
-    }
-#pragma unroll 1
-    for (int c = 0; c < kD / 32; ++c) {
-      uint32_t v[32];
-      if (n_tiles > 0) {
-        tmem_ld_32x32b_x32(o_tmem + c * 32, v);
-        tmem_ld_wait();
-      } else {
-#pragma unroll
-        for (int i = 0; i < 32; ++i) v[i] = 0;
-      }
-      if (dst) {
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          uint4 o;
-          o.x = pack_bf16x2(__uint_as_float(v[8 * i + 0]) * inv, __uint_as_float(v[8 * i + 1]) * inv);
-          o.y = pack_bf16x2(__uint_as_float(v[8 * i + 2]) * inv, __uint_as_float(v[8 * i + 3]) * inv);
-          o.z = pack_bf16x2(__uint_as_float(v[8 * i + 4]) * inv, __uint_as_float(v[8 * i + 5]) * inv);
-          o.w = pack_bf16x2(__uint_as_float(v[8 * i + 6]) * inv, __uint_as_float(v[8 * i + 7]) * inv);
-          *reinterpret_cast<uint4*>(dst + c * 32 + i * 8) = o;
-        }
-      }
-    }
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc(tmem_base, Cfg::kTmemCols);
 }
 
 // Combines the kv_splits partials of every (q row, head): weights 2^(lse_s - max) / sum, fixed split order.
@@ -780,55 +322,17 @@ static int launch_prefill(const CUtensorMap& tq, const CUtensorMap& tk, const CU
     XB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
     attr_done = true;
   }
-  dim3 grid(q_tiles, p.num_kv_heads, batch * p.kv_splits), block(192);
+  dim3 grid(q_tiles, p.num_kv_heads, batch * p.kv_splits), block(kPrefillThreads);
   XB_CUDA_OK(launch(kern, grid, block, (size_t)Cfg::kSmemBytes, stream, true, tq, tk, tv, p));
   if (p.kv_splits > 1)
     XB_CUDA_OK(launch(prefill_merge_kernel, dim3((unsigned)p.total_q, p.num_qo_heads), dim3(kD < 128 ? kD : 128), 0, stream, true, p, kD));
   return 0;
 }
-
-template <int kD>
-static int launch_prefill2(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const PrefillParams& p,
-                           int batch, int q_tiles, cudaStream_t stream) {
-  using Cfg = Prefill2Cfg<kD>;
-  auto kern = prefill_attention2_kernel<kD>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    XB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_done = true;
-  }
-  dim3 grid((q_tiles + 1) / 2, p.num_kv_heads, batch), block(Cfg::kThreads);
-  XB_CUDA_OK(launch(kern, grid, block, (size_t)Cfg::kSmemBytes, stream, true, tq, tk, tv, p));
-  return 0;
-}
-
 }  // namespace tc
 }  // namespace xb
 
 using namespace xb;
 using namespace xb::tc;
-
-// 0: one q tile per CTA (prefill_attention_kernel); 1: two q tiles per CTA, two softmax warpgroups (ping-pong).  Split-KV
-// launches always take variant 0.
-static std::atomic<int> g_prefill_variant{-1};
-static int prefill_variant() {
-  int v = g_prefill_variant.load(std::memory_order_relaxed);
-  if (v < 0) {
-    const char* e = getenv("XB_PREFILL_V2");
-    v = e ? (atoi(e) != 0) : 1;     // measured on B200 (4 x 2048 causal, 28 / 4 heads of 128): 574 vs 465 TF/s, bit-identical
-    g_prefill_variant.store(v, std::memory_order_relaxed);
-  }
-  return v;
-}
-extern "C" int xb_set_prefill_variant(int variant) {
-  if (variant < 0 || variant > 1) {
-    set_error("set_prefill_variant: variant %d (0 one q tile per CTA | 1 ping-pong pair)", variant);
-    return -1;
-  }
-  const int old = prefill_variant();
-  g_prefill_variant.store(variant, std::memory_order_relaxed);
-  return old;
-}
 
 // Shared host path of ragged_run / paged_run.
 static int prefill_common(const void* q, int64_t q_stride_n, int64_t q_stride_h, int64_t total_q, const void* k,
@@ -875,12 +379,6 @@ static int prefill_common(const void* q, int64_t q_stride_n, int64_t q_stride_h,
   p.causal = causal;
   p.kv_splits = kv_splits;
   p.total_q = total_q;
-  static const float tau = [] { const char* e = getenv("XB_PREFILL_TAU"); return e ? (float)atof(e) : 0.f; }();
-  p.rescale_tau = tau;
-  static const int qk_first = [] { const char* e = getenv("XB_PREFILL_QK_FIRST"); return e ? atoi(e) : 1; }();   // measured +2.4 % (551 -> 565 TF/s), bit-identical
-  static const int spin_mma = [] { const char* e = getenv("XB_PREFILL_SPIN"); return e ? atoi(e) : 0; }();
-  p.qk_first = qk_first;
-  p.spin_mma = spin_mma;
   p.part_o = reinterpret_cast<float*>(workspace_f32);
   p.part_lse = p.part_o ? p.part_o + (int64_t)kv_splits * total_q * num_qo_heads * head_dim : nullptr;
   if (paged) {
@@ -897,9 +395,6 @@ static int prefill_common(const void* q, int64_t q_stride_n, int64_t q_stride_h,
   if (make_tmap_2d(&tk, k, kv_rows, (uint64_t)num_kv_heads * head_dim, (uint64_t)kv_row_stride * 2, p.box_rows, 64, 2)) return 1;
   if (make_tmap_2d(&tv, v, kv_rows, (uint64_t)num_kv_heads * head_dim, (uint64_t)kv_row_stride * 2, p.box_rows, 64, 2)) return 1;
   const int q_tiles = (max_qo_len + p.tokens_per_tile - 1) / p.tokens_per_tile;
-  if (kv_splits == 1 && q_tiles >= 2 && prefill_variant() == 1)
-    return head_dim == 128 ? launch_prefill2<128>(tq, tk, tv, p, batch, q_tiles, stream)
-                           : launch_prefill2<64>(tq, tk, tv, p, batch, q_tiles, stream);
   return head_dim == 128 ? launch_prefill<128>(tq, tk, tv, p, batch, q_tiles, stream)
                          : launch_prefill<64>(tq, tk, tv, p, batch, q_tiles, stream);
 }
@@ -953,7 +448,7 @@ extern "C" int64_t xb_prefill_split_workspace_bytes(int kv_splits, int64_t total
 extern "C" int xb_prefill_plan_splits(int batch, int max_qo_len, int64_t max_kv_len, int num_qo_heads, int num_kv_heads,
                                       int num_sms) {
   if (batch <= 0 || max_qo_len <= 0 || num_kv_heads <= 0 || num_qo_heads % num_kv_heads != 0) return 1;
-  if (num_sms <= 0) num_sms = 148;
+  if (num_sms <= 0) num_sms = 132;
   const int group = num_qo_heads / num_kv_heads;
   const int tokens_per_tile = group <= 128 ? 128 / group : 1;
   const int64_t q_tiles = (max_qo_len + tokens_per_tile - 1) / tokens_per_tile;

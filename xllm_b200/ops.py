@@ -34,12 +34,10 @@ def _cuda_bf16(t, name):
     _need(t.dtype == BF16, f"{name} must be bfloat16, got {t.dtype}")
 
 
-# Streaming (small-M) kernels vs the 128-row tcgen05 GEMMs, measured on B200 (tools/gemv_sweep.py q8, us per call):
-#   the GEMMs launch one CTA per 128 x 256 (fp8) / 128 x 128..256 (weight-only) output tile, so with few output columns most
-#   SMs idle; weight-only, M = 32: N 3584 44 vs 122, N 10240 49 vs 106, N 37888 52 vs 35; M = 64: 93 vs 122, 102 vs 106, 119 vs 36
-#   => weight-only: streaming up to M = 16 always, up to M = 64 when N <= 16384.
-#   fp8: M = 1: N 10240 41.6 vs 49.3, N 3584 32 vs 54, N 37888 63 vs 32; M = 32: 54 vs 43, 58 vs 48, 86 vs 32
-#   => fp8: streaming only up to M = 8 and N <= 16384 (the tcgen05 FP8 kernel streams 1 byte per weight already).
+# Streaming (small-M) kernels vs the 128-row GEMMs: the GEMMs launch one CTA per 128-row output tile, so with few output
+# columns most SMs idle, while the streaming kernels spread every weight row over the SMs.  Weight-only: streaming up to
+# M = 16 always, up to M = 64 when N <= 16384.  FP8: streaming only up to M = 8 and N <= 16384 (the FP8 GEMM's swap-AB
+# form already streams 1 byte per weight).  The crossovers have not been re-measured on the H100 (tools/gemv_sweep.py q8).
 FP8_SMALL_M_MAX = 8
 WQ_SMALL_M_MAX = 16
 WQ_SMALL_M_MAX_NARROW = 64      # ... when the projection has at most SMALL_N_MAX output columns
@@ -301,10 +299,10 @@ def argmax(out, logits) -> None:
                                c_i32(logits.size(1)), _stream()), "argmax")
 
 
-# ---- tcgen05 GEMMs ---------------------------------------------------------------
+# ---- wgmma GEMMs ---------------------------------------------------------------
 def matmul(a, b, bias=None, out=None):
     """xllm::kernel::cuda::matmul (cuda_ops_api.h:167-169): F::linear(a, b, bias); a [M,K], b [N,K] bf16.
-    M <= 16 streams the weight once through the small-M kernel; larger M runs the tcgen05 GEMM."""
+    M <= 16 streams the weight once through the small-M kernel; larger M runs the wgmma GEMM."""
     _cuda_bf16(a, "a"); _cuda_bf16(b, "b")
     M, K = a.shape
     N = b.size(0)
@@ -315,12 +313,6 @@ def matmul(a, b, bias=None, out=None):
     check(lib().xb_gemm_bf16(_p(y), c_i64(y.stride(0)), _p(a), c_i64(a.stride(0)), _p(b), _p(bias), c_i32(M), c_i32(N),
                              c_i32(K), _stream()), "matmul")
     return y
-
-
-def set_gemm_cta_pair(mode: int) -> int:
-    """kernel selection of the tcgen05 GEMMs: 0 auto | 1 single-CTA | 2 CTA pairs (cta_group::2) when >= 74 pair tiles |
-    3 CTA pairs whenever M > 128 and N % 256 == 0.  Returns the previous mode."""
-    return int(lib().xb_set_gemm_cta_pair(c_i32(mode)))
 
 
 def set_fp8_swap_max_m(max_m: int) -> int:
@@ -358,7 +350,7 @@ def set_fp8_splitk_max(max_split: int) -> int:
 
 
 def gemm_fp8_scaled(c, a, w, a_scales, b_scales, bias=None) -> None:
-    """the tcgen05 FP8 kernel directly (no small-M dispatch): a [M,K] e4m3, w [N,K] e4m3 (the reference's weight layout)."""
+    """the wgmma FP8 kernel directly (no small-M dispatch): a [M,K] e4m3, w [N,K] e4m3 (the reference's weight layout)."""
     M, K = a.shape
     N = w.size(0)
     check(lib().xb_gemm_fp8_scaled(_p(c), c_i64(c.stride(0)), _p(a), c_i64(a.stride(0)), _p(w), _p(a_scales),
@@ -367,7 +359,7 @@ def gemm_fp8_scaled(c, a, w, a_scales, b_scales, bias=None) -> None:
 
 
 def gemm_bf16(a, b, bias=None, out=None):
-    """always the tcgen05 kernel (tests / benchmarks)."""
+    """always the wgmma kernel (tests / benchmarks)."""
     _cuda_bf16(a, "a"); _cuda_bf16(b, "b")
     M, K = a.shape
     N = b.size(0)
@@ -424,7 +416,7 @@ def fp8_scaled_matmul(a, b, a_scale, b_scale, output_dtype=BF16, bias=None, outp
 
 
 def w4a16_linear(x, qweight, meta, group_size, bias=None, out=None):
-    """weight-only linear for any M: small-M streaming kernel up to 16 tokens, tcgen05 dequant-GEMM above."""
+    """weight-only linear for any M: small-M streaming kernel up to 16 tokens, wgmma dequant-GEMM above."""
     _cuda_bf16(x, "x")
     M, K = x.shape
     N = meta.size(1)
@@ -437,7 +429,7 @@ def w4a16_linear(x, qweight, meta, group_size, bias=None, out=None):
 
 
 def gemm_w4a16(x, qweight, meta, group_size, bias=None, out=None):
-    """always the tcgen05 dequant-GEMM (tests / benchmarks)."""
+    """always the wgmma dequant-GEMM (tests / benchmarks)."""
     _cuda_bf16(x, "x")
     M, K = x.shape
     N = meta.size(1)
@@ -448,11 +440,6 @@ def gemm_w4a16(x, qweight, meta, group_size, bias=None, out=None):
 
 
 # ---- K3 / K2 prefill attention ------------------------------------------------------
-def set_prefill_variant(variant: int) -> int:
-    """0: one q tile per CTA; 1: ping-pong pair of q tiles with two softmax warpgroups.  Returns the old variant."""
-    return int(lib().xb_set_prefill_variant(c_i32(variant)))
-
-
 
 def batch_prefill(query, key, value, q_cu_seq_lens, kv_cu_seq_lens, sm_scale, output, output_lse=None, max_qo_len=None,
                   causal=True) -> None:
@@ -474,7 +461,7 @@ def batch_prefill(query, key, value, q_cu_seq_lens, kv_cu_seq_lens, sm_scale, ou
           "batch_prefill")
 
 
-def prefill_plan_splits(batch, max_qo_len, max_kv_len, num_qo_heads, num_kv_heads, num_sms=148) -> int:
+def prefill_plan_splits(batch, max_qo_len, max_kv_len, num_qo_heads, num_kv_heads, num_sms=132) -> int:
     """host-side split-KV decision for a short query chunk over a long KV (what the reference's prefill `plan` decides,
     flashinfer_planinfo.cpp:168-247)."""
     return int(lib().xb_prefill_plan_splits(c_i32(batch), c_i32(max_qo_len), c_i64(max_kv_len), c_i32(num_qo_heads),
@@ -517,7 +504,7 @@ def batch_chunked_prefill(query, k_cache, v_cache, paged_kv_indptr, paged_kv_ind
 
 def w4a16_gate_up_act(x, qweight, meta, group_size, act_mode="silu", bias=None, out=None, gate_up_buf=None):
     """DenseMLPImpl's gate_up linear + act_and_mul (dense_mlp.cpp:97-118) with the INTERLEAVED gate/up packing
-    (quant.pack_w4_gate_up).  M <= 16: one fused kernel (activation in the GEMV epilogue); larger M: tcgen05
+    (quant.pack_w4_gate_up).  M <= 16: one fused kernel (activation in the GEMV epilogue); larger M: wgmma
     dequant-GEMM into `gate_up_buf` + act_and_mul over the interleaved columns."""
     _cuda_bf16(x, "x")
     if act_mode not in _ACT:
@@ -623,7 +610,7 @@ def w8a16_linear_small_m(x, qweight, meta, group_size, bias=None, out=None):
 
 
 def gemm_w8a16(x, qweight, meta, group_size, bias=None, out=None):
-    """always the tcgen05 dequant-GEMM (tests / benchmarks)."""
+    """always the wgmma dequant-GEMM (tests / benchmarks)."""
     _cuda_bf16(x, "x")
     M, K = x.shape
     N = meta.size(1)
@@ -634,7 +621,7 @@ def gemm_w8a16(x, qweight, meta, group_size, bias=None, out=None):
 
 
 def w8a16_linear(x, qweight, meta, group_size, bias=None, out=None):
-    """weight-only int8 linear for any M: streaming kernel for decode batches, tcgen05 dequant-GEMM above."""
+    """weight-only int8 linear for any M: streaming kernel for decode batches, wgmma dequant-GEMM above."""
     M, N = x.shape[0], meta.size(1)
     if M <= WQ_SMALL_M_MAX or (M <= WQ_SMALL_M_MAX_NARROW and N <= SMALL_N_MAX):
         return w8a16_linear_small_m(x, qweight, meta, group_size, bias, out)

@@ -68,7 +68,7 @@ def pack_w4_qkv_rope(q, scales, zeros, num_heads, num_kv_heads, head_dim, group_
 def pack_w8(q: torch.Tensor, scales: torch.Tensor, zeros: torch.Tensor, group_size: int = 128):
     """W8A16: q uint8 [N,K] in 0..255 -> (qweight int32 [N/16,K/64,32,8], meta int32 [K/g,N] = bf16 scale | zero << 16).
     Lane 4g+t of a 16x64 tile holds rows g (words 0..3) and g+8 (words 4..7), k in [16t, 16t+16) ascending
-    (csrc/linear_q8_small_m.cu; the same tensor feeds the tcgen05 GEMM kind W8)."""
+    (csrc/linear_q8_small_m.cu; the same tensor feeds the wgmma GEMM kind W8)."""
     N, K = q.shape
     assert N % 16 == 0 and K % 64 == 0 and K % group_size == 0 and group_size % 64 == 0
     qq = q.to(torch.int32).view(N // 16, 2, 8, K // 64, 4, 4, 4)          # [nt, half, g, kt, t, j, byte]

@@ -102,7 +102,7 @@ class Linear:
         return self.qweight.numel() * 4 + self.meta.numel() * 4
 
     def forward(self, x, out):
-        """M <= 16: HBM-bound streaming kernels; larger M: tcgen05 GEMMs.  fp8 follows fp8_linear_forward
+        """M <= 16: HBM-bound streaming kernels; larger M: wgmma GEMMs.  fp8 follows fp8_linear_forward
         (linear.cpp:137-182): quantise the activation (static scale if present) then the scaled matmul."""
         if self.kind == "bf16":
             ops.matmul(x, self.weight, self.bias, out)
@@ -239,9 +239,8 @@ class Qwen2DecodeRunner:
         """pg: xllm_b200.parallel.ProcessGroup for tensor parallelism (weights must already be this rank's shards);
         exchange: "peer" = NVLink one-shot all-reduce fused with add+RMSNorm, "nccl" = c10d all-reduce (baseline);
         fuse_gemv: W4A16 decode with batch <= 8 splits add+RMSNorm between the o / down epilogues and the qkv / gate_up
-        prologues (5 launches per layer instead of 7).  OFF by default: measured on B200 (profiles/r02a_*) the 145-launch
-        step runs at 1.90 ms against 1.74 ms for the 200-launch step whose small add+RMSNorm kernels overlap the next
-        GEMV's weight prefetch under PDL.  RoPE + KV scatter (qkv epilogue) and SiLU*mul (gate_up epilogue) ride in the
+        prologues (5 launches per layer instead of 7).  OFF by default: the 200-launch step's small add+RMSNorm kernels
+        overlap the next GEMV's weight prefetch under PDL, while folded into the GEMVs they sit on every CTA's critical path.  RoPE + KV scatter (qkv epilogue) and SiLU*mul (gate_up epilogue) ride in the
         GEMVs either way."""
         self.cfg, self.w, self.B, self.device = cfg, weights, max_batch, device
         self.pg = pg if (pg is not None and pg.world_size > 1) else None
@@ -321,7 +320,7 @@ class Qwen2DecodeRunner:
                                all(L[k].input_scale is not None for L in weights.layers for k in ("qkv", "gate_up")))
         self.normed8 = torch.empty(B, H, dtype=torch.float8_e4m3fn, device=dev) if cfg.quant == "fp8" else None
         if cfg.quant == "fp8" and os.environ.get("XB_FP8_SPLITK", "1") != "0":
-            # decode-sized FP8 linears: K split over otherwise idle SMs (shard-sized N leaves 10-64 weight tiles for 148 SMs)
+            # decode-sized FP8 linears: K split over otherwise idle SMs (shard-sized N leaves 10-64 weight tiles for 132 SMs)
             ops.enable_fp8_splitk(dev)
         self.embed_local = torch.empty(B, weights.embed.size(1), dtype=BF16, device=dev) if weights.embed.size(1) != H else None
         self.plan = ops.DecodePlan(B, self.nh, self.nkv, cfg.head_dim, bs, self.max_pages, dev, early_prefetch=True)
