@@ -8,6 +8,7 @@
 #include <atomic>
 #include <cstdarg>
 #include <cstdio>
+#include <utility>
 
 #include "../../include/xllm_b200_ops.h"
 
@@ -36,36 +37,11 @@ extern std::atomic<int> g_pdl_enabled;
     }                                                                         \
   } while (0)
 
-// Experiment switch (OFF by default): XB_SMEM_CARVEOUT=1 makes every kernel ask for the maximum shared-memory carveout,
-// so that consecutive kernels of a decode step never re-partition the SM.  Off by default: the streaming kernels want the
-// L1 that the driver's per-kernel heuristic leaves them.
-void prefer_max_shared_carveout(const void* kernel);
+// SM count of the device current at the first call, cached for the process.
+int device_sm_count();
 
-// Launch helper: counts launches, optionally attaches the PDL attribute.
-template <typename... KArgs, typename... Args>
-inline cudaError_t launch(void (*kernel)(KArgs...), dim3 grid, dim3 block,
-                          size_t smem, cudaStream_t stream, bool pdl,
-                          Args&&... args) {
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = grid;
-  cfg.blockDim = block;
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  int n = 0;
-  if (pdl && g_pdl_enabled.load(std::memory_order_relaxed)) {
-    attr[n].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[n].val.programmaticStreamSerializationAllowed = 1;
-    ++n;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = n;
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  prefer_max_shared_carveout(reinterpret_cast<const void*>(kernel));
-  return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
-}
-
-// Same, as a thread-block-cluster launch (cluster_x CTAs along grid x; 1 = plain launch).
+// Launch helper: counts launches, optionally attaches the PDL attribute, launches thread-block clusters of cluster_x CTAs
+// along grid x (1 = plain launch).
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
                                   bool pdl, int cluster_x, Args&&... args) {
@@ -91,8 +67,20 @@ inline cudaError_t launch_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 bloc
   cfg.attrs = attr;
   cfg.numAttrs = n;
   g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  prefer_max_shared_carveout(reinterpret_cast<const void*>(kernel));
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream, bool pdl,
+                          Args&&... args) {
+  return launch_cluster(kernel, grid, block, smem, stream, pdl, 1, std::forward<Args>(args)...);
+}
+
+// Raises kKernel's dynamic shared-memory limit to `bytes` once per process, on the device current at the first call;
+// every call returns the result of that one attempt.
+template <auto kKernel>
+inline cudaError_t set_max_dynamic_smem_once(int bytes) {
+  static const cudaError_t err = cudaFuncSetAttribute(kKernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  return err;
 }
 
 // ---- device helpers ---------------------------------------------------------
@@ -213,6 +201,35 @@ __device__ __forceinline__ uint32_t hmul2_bf16x2(uint32_t a, uint32_t b) {
   asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
   return d;
 }
+__device__ __forceinline__ uint32_t hsub2_bf16x2(uint32_t a, uint32_t b) {
+  uint32_t d;
+  asm("sub.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
+  return d;
+}
+// int4 weight-only dequant (oracle/quant.py, bits = 4) of the tile-packed W4 layout described in linear_small_m.cu.
+// W4 meta word (bf16 scale | bf16(128 + zero) << 16) -> bf16x2 scale, bf16x2 (128 + zero)
+__device__ __forceinline__ void w4_meta(uint32_t m, uint32_t& s2, uint32_t& z2) {
+  s2 = __byte_perm(m, 0, 0x1010);
+  z2 = __byte_perm(m, 0, 0x3232);
+}
+// one packed word -> the four bf16x2 mma A-fragment registers as exact bf16 integers 128 + q: (w >> 4i) & 0x000f000f | 0x4300
+// in each half; q[0] / q[2] are row g, q[1] / q[3] row g+8
+__device__ __forceinline__ void w4_nibbles(uint32_t w, uint32_t (&q)[4]) {
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+    asm("lop3.b32 %0, %1, %2, %3, 0xea;" : "=r"(q[i]) : "r"(w >> (4 * i)), "r"(0x000f000fu), "r"(0x43004300u));  // (a & b) | c
+}
+// w = bf16((q - z) * s), bit-exact with the spec: (128 + q) - (128 + z) is exact, the product by s rounds once.
+// a[0] / a[2] are row g (scale s0, zero z0), a[1] / a[3] row g+8 (s1, z1).
+__device__ __forceinline__ void w4_dequant_word(uint32_t w, uint32_t z0, uint32_t s0, uint32_t z1, uint32_t s1,
+                                                uint32_t (&a)[4]) {
+  uint32_t q[4];
+  w4_nibbles(w, q);
+  a[0] = hmul2_bf16x2(hsub2_bf16x2(q[0], z0), s0);
+  a[1] = hmul2_bf16x2(hsub2_bf16x2(q[1], z1), s1);
+  a[2] = hmul2_bf16x2(hsub2_bf16x2(q[2], z0), s0);
+  a[3] = hmul2_bf16x2(hsub2_bf16x2(q[3], z1), s1);
+}
 // int8 weight-only dequant (oracle/quant.py, bits = 8): four unsigned bytes of one weight row (k ascending) -> two bf16x2
 // registers bf16((q - z) * s), bit-exact with the spec: 0x4B0000qq is float(2^23 + q), adding neg_mz = -(2^23 + z) gives
 // q - z exactly, the bf16x2 pack is exact for |q - z| <= 255 and the product by s rounds once.
@@ -251,6 +268,15 @@ __device__ __forceinline__ void mma_bf16_16816(float (&c)[4], uint32_t a0,
       "{%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
       : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
       : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
+// C fragment of lane (g, t) of an m16n8 mma into a row-major 16 x 8 fp32 tile:
+// c0 (g, 2t), c1 (g, 2t+1), c2 (g+8, 2t), c3 (g+8, 2t+1)
+__device__ __forceinline__ void store_c_frag(float* tile16x8, const float (&c)[4], int g, int t) {
+  tile16x8[g * 8 + 2 * t] = c[0];
+  tile16x8[g * 8 + 2 * t + 1] = c[1];
+  tile16x8[(g + 8) * 8 + 2 * t] = c[2];
+  tile16x8[(g + 8) * 8 + 2 * t + 1] = c[3];
 }
 
 #endif  // __CUDACC__

@@ -434,28 +434,21 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
               w8_dequant_word(bv[j], nz1, s1, hi[2 * j], hi[2 * j + 1]);
             }
           } else {
-          const uint4 wq = lds_128(pk + r * 512 + lane * 16);
-          const uint32_t s0 = __byte_perm(m0, 0, 0x1010), z0 = __byte_perm(m0, 0, 0x3232);
-          const uint32_t s1 = __byte_perm(m1, 0, 0x1010), z1 = __byte_perm(m1, 0, 0x3232);
-          const uint32_t* wv = &wq.x;
+            // int4 tile: 16 bytes per lane in the layout of linear_small_m.cu (common.cuh w4_dequant_word)
+            const uint4 wq = lds_128(pk + r * 512 + lane * 16);
+            uint32_t s0, z0, s1, z1;
+            w4_meta(m0, s0, z0);
+            w4_meta(m1, s1, z1);
+            const uint32_t* wv = &wq.x;
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const uint32_t w = wv[j];
-            uint32_t q0, q1, q2, q3;
-            asm("lop3.b32 %0, %1, 0x000f000f, 0x43004300, 0xea;" : "=r"(q0) : "r"(w));
-            asm("lop3.b32 %0, %1, 0x000f000f, 0x43004300, 0xea;" : "=r"(q1) : "r"(w >> 4));
-            asm("lop3.b32 %0, %1, 0x000f000f, 0x43004300, 0xea;" : "=r"(q2) : "r"(w >> 8));
-            asm("lop3.b32 %0, %1, 0x000f000f, 0x43004300, 0xea;" : "=r"(q3) : "r"(w >> 12));
-            uint32_t d;
-            asm("sub.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(q0), "r"(z0));
-            asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(lo[2 * j]) : "r"(d), "r"(s0));
-            asm("sub.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(q2), "r"(z0));
-            asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(lo[2 * j + 1]) : "r"(d), "r"(s0));
-            asm("sub.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(q1), "r"(z1));
-            asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(hi[2 * j]) : "r"(d), "r"(s1));
-            asm("sub.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(q3), "r"(z1));
-            asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(hi[2 * j + 1]) : "r"(d), "r"(s1));
-          }
+            for (int j = 0; j < 4; ++j) {
+              uint32_t a[4];
+              w4_dequant_word(wv[j], z0, s0, z1, s1, a);
+              lo[2 * j] = a[0];
+              hi[2 * j] = a[1];
+              lo[2 * j + 1] = a[2];
+              hi[2 * j + 1] = a[3];
+            }
           }
           // swizzled K-major tile: row n at n*128 bytes, 16-byte chunk c stored at chunk (c ^ (n & 7))
           const int n_lo = r * 16 + g, n_hi = n_lo + 8;
@@ -478,16 +471,9 @@ template <int kKind, int kBlockN>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p, cudaStream_t stream,
                        const CUtensorMap* tm = nullptr) {
   using Cfg = GemmCfg<kKind, kBlockN>;
-  auto kern = gemm_wgmma_kernel<kKind, kBlockN>;
-  static bool attr_done = false;
-  static int max_ctas = 132;     // persistent CTAs: one per SM
-  if (!attr_done) {
-    XB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&max_ctas, cudaDevAttrMultiProcessorCount, dev);
-    attr_done = true;
-  }
+  constexpr auto kern = gemm_wgmma_kernel<kKind, kBlockN>;
+  XB_CUDA_OK(set_max_dynamic_smem_once<kern>(Cfg::kSmemBytes));
+  const int max_ctas = device_sm_count();     // persistent CTAs: one per SM
   if (p.split_k < 1) p.split_k = 1;
   const int units = ((p.M + kBlockM - 1) / kBlockM) * ((p.N + kBlockN - 1) / kBlockN) * p.split_k;
   dim3 grid(units < max_ctas ? units : max_ctas), block(Cfg::kThreads);
@@ -510,8 +496,6 @@ static int make_tmap_fp8(CUtensorMap* out, const void* base, uint64_t rows, uint
 // the 132 SMs about once, 64-column tiles below that (the reference buckets by M the same way)
 static int pick_block_n(int M, int N) {
   const int m_blocks = (M + kBlockM - 1) / kBlockM;
-  static const int force = [] { const char* e = getenv("XB_GEMM_BN"); return e ? atoi(e) : 0; }();
-  if (force == 64 || force == 128) return force;
   if ((int64_t)m_blocks * ((N + 127) / 128) >= 120) return 128;
   return 64;
 }
@@ -566,8 +550,7 @@ static int pick_split_k(int tiles, int num_kb, int tokens_bn, size_t* need_bytes
     cudaGetLastError();
     return 1;
   }
-  static int sms = [] { int d = 0, n = 132; cudaGetDevice(&d); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d); return n; }();
-  int split = split_k_for(tiles, num_kb, sms);
+  int split = split_k_for(tiles, num_kb, device_sm_count());
   if (split < 2) return 1;
   const size_t need = kSplitKTicketBytes + (size_t)tiles * split * tokens_bn * kBlockM * sizeof(float);
   if ((size_t)tiles * sizeof(unsigned) > kSplitKTicketBytes || need > g_splitk_bytes.load(std::memory_order_relaxed)) return 1;

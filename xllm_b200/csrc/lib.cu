@@ -1,10 +1,5 @@
-// Library-level plumbing of libxllm_b200_ops.so: error string, launch counter, PDL switch.
+// Library-level plumbing of libxllm_b200_ops.so: error string, launch counter, PDL switch, SM count.
 #include "common.cuh"
-
-#include <cstdlib>
-#include <cstring>
-#include <mutex>
-#include <unordered_set>
 
 namespace xb {
 std::atomic<uint64_t> g_launch_count{0};
@@ -16,16 +11,14 @@ void set_error(const char* fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
 }
-void prefer_max_shared_carveout(const void* kernel) {
-  static const bool enabled = [] { const char* e = getenv("XB_SMEM_CARVEOUT"); return e && atoi(e) != 0; }();
-  if (!enabled) return;
-  static std::mutex mu;
-  static std::unordered_set<const void*> done;
-  std::lock_guard<std::mutex> lock(mu);
-  if (done.insert(kernel).second) {
-    cudaFuncSetAttribute(kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared);
-    cudaGetLastError();
-  }
+int device_sm_count() {
+  static const int sms = [] {
+    int d = 0, n = 132;
+    cudaGetDevice(&d);
+    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d);
+    return n;
+  }();
+  return sms;
 }
 }  // namespace xb
 

@@ -116,12 +116,7 @@ linear_w8a16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, con
   pdl_launch_dependents();
 
 #pragma unroll
-  for (int m = 0; m < kMT; ++m) {
-    red[warp][m][g * 8 + 2 * t] = acc[m][0];
-    red[warp][m][g * 8 + 2 * t + 1] = acc[m][1];
-    red[warp][m][(g + 8) * 8 + 2 * t] = acc[m][2];
-    red[warp][m][(g + 8) * 8 + 2 * t + 1] = acc[m][3];
-  }
+  for (int m = 0; m < kMT; ++m) store_c_frag(red[warp][m], acc[m], g, t);
   __syncthreads();
   for (int i = threadIdx.x; i < kMT * 128; i += blockDim.x) {
     const int m = i >> 7, r = (i & 127) >> 3, c = i & 7;
@@ -191,12 +186,7 @@ linear_fp8_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, const
   if (ktiles <= warp) pdl_wait();
   pdl_launch_dependents();
 #pragma unroll
-  for (int m = 0; m < kMT; ++m) {
-    red[warp][m][g * 8 + 2 * t] = acc[m][0];
-    red[warp][m][g * 8 + 2 * t + 1] = acc[m][1];
-    red[warp][m][(g + 8) * 8 + 2 * t] = acc[m][2];
-    red[warp][m][(g + 8) * 8 + 2 * t + 1] = acc[m][3];
-  }
+  for (int m = 0; m < kMT; ++m) store_c_frag(red[warp][m], acc[m], g, t);
   __syncthreads();
   for (int i = threadIdx.x; i < kMT * 128; i += blockDim.x) {
     const int m = i >> 7, r = (i & 127) >> 3, c = i & 7;
@@ -241,12 +231,8 @@ extern "C" int xb_linear_w8a16_small_m(void* y, int64_t y_stride, const void* x,
   constexpr size_t smem = (size_t)kQ8Warps * kDepth * (1024 + 256);
 #define XB_W8(MT)                                                                                                   \
   {                                                                                                                 \
-    auto kern = linear_w8a16_small_m_kernel<MT, kDepth>;                                                            \
-    static bool attr_done = false;                                                                                  \
-    if (!attr_done) {                                                                                               \
-      XB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));               \
-      attr_done = true;                                                                                             \
-    }                                                                                                               \
+    constexpr auto kern = linear_w8a16_small_m_kernel<MT, kDepth>;                                                  \
+    XB_CUDA_OK(set_max_dynamic_smem_once<kern>((int)smem));                                                         \
     XB_CUDA_OK(launch(kern, grid, block, smem, s, true, yy, y_stride, xx, x_stride, qw, meta, bb, M, N, K, gshift)); \
   }
   if (M <= 8) XB_W8(1)

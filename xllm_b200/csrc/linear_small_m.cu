@@ -31,22 +31,6 @@ namespace xb {
 
 constexpr int kWarps = 8;
 
-__device__ __forceinline__ uint32_t hsub2_bf16(uint32_t a, uint32_t b) {
-  uint32_t d;
-  asm("sub.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
-  return d;
-}
-__device__ __forceinline__ uint32_t hmul2_bf16(uint32_t a, uint32_t b) {  // (same as hmul2_bf16x2 in common.cuh)
-  uint32_t d;
-  asm("mul.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
-  return d;
-}
-__device__ __forceinline__ uint32_t lop3_and_or(uint32_t a, uint32_t mask, uint32_t orv) {
-  uint32_t d;
-  asm("lop3.b32 %0, %1, %2, %3, 0xea;" : "=r"(d) : "r"(a), "r"(mask), "r"(orv));  // (a & b) | c
-  return d;
-}
-
 // m16n8k16 with a zero accumulator input (opens a fresh accumulation chain without clearing registers)
 __device__ __forceinline__ void mma_bf16_16816_zero(float (&c)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3,
                                                     uint32_t b0, uint32_t b1) {
@@ -356,8 +340,9 @@ linear_w4a16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, con
 #pragma unroll
     for (int u = 0; u < kTG; ++u) wq[u] = lds_128(ring_w + i * kSlotBytes + u * 512);
     const uint2 mt = lds_64(ring_m + i * kSlotBytes);
-    const uint32_t s0 = __byte_perm(mt.x, 0, 0x1010), z0 = __byte_perm(mt.x, 0, 0x3232);
-    const uint32_t s1 = __byte_perm(mt.y, 0, 0x1010), z1 = __byte_perm(mt.y, 0, 0x3232);
+    uint32_t s0, z0, s1, z1;
+    w4_meta(mt.x, s0, z0);
+    w4_meta(mt.y, s1, z1);
 #pragma unroll
     for (int u = 0; u < kTG; ++u) {
       const int par = (i * kTG + u) & 1;       // compile-time after unrolling (kDepth * kTG is even)
@@ -367,20 +352,13 @@ linear_w4a16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, con
       const uint32_t* wv = &wq[u].x;
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        const uint32_t w = wv[j];
-        const uint32_t q0 = lop3_and_or(w, 0x000f000fu, 0x43004300u);
-        const uint32_t q1 = lop3_and_or(w >> 4, 0x000f000fu, 0x43004300u);
-        const uint32_t q2 = lop3_and_or(w >> 8, 0x000f000fu, 0x43004300u);
-        const uint32_t q3 = lop3_and_or(w >> 12, 0x000f000fu, 0x43004300u);
-        const uint32_t a0 = hmul2_bf16(hsub2_bf16(q0, z0), s0);
-        const uint32_t a1 = hmul2_bf16(hsub2_bf16(q1, z1), s1);
-        const uint32_t a2 = hmul2_bf16(hsub2_bf16(q2, z0), s0);
-        const uint32_t a3 = hmul2_bf16(hsub2_bf16(q3, z1), s1);
+        uint32_t a[4];
+        w4_dequant_word(wv[j], z0, s0, z1, s1, a);
 #pragma unroll
         for (int m = 0; m < kMT; ++m) {
           // lane run element 4j+{0,1} -> b0, 4j+{2,3} -> b1
           const uint32_t* xv = j < 2 ? &xf.lo[m].x : &xf.hi[m].x;
-          mma_bf16_16816(accj[j % kAcc][m], a0, a1, a2, a3, xv[(j & 1) * 2], xv[(j & 1) * 2 + 1]);
+          mma_bf16_16816(accj[j % kAcc][m], a[0], a[1], a[2], a[3], xv[(j & 1) * 2], xv[(j & 1) * 2 + 1]);
         }
       }
     }
@@ -404,17 +382,14 @@ linear_w4a16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, con
       const uint32_t* wv = &wq[u].x;
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        const uint32_t w = wv[j];
-        const uint32_t q0 = lop3_and_or(w, 0x000f000fu, 0x43004300u);
-        const uint32_t q1 = lop3_and_or(w >> 4, 0x000f000fu, 0x43004300u);
-        const uint32_t q2 = lop3_and_or(w >> 8, 0x000f000fu, 0x43004300u);
-        const uint32_t q3 = lop3_and_or(w >> 12, 0x000f000fu, 0x43004300u);
+        uint32_t q[4];
+        w4_nibbles(wv[j], q);
         const uint32_t* xv = j < 2 ? &xf.lo[0].x : &xf.hi[0].x;
         const uint32_t b0 = xv[(j & 1) * 2], b1 = xv[(j & 1) * 2 + 1];
-        if (u == 0 && j == 0) mma_bf16_16816_zero(c0, q0, q1, q2, q3, b0, b1);
-        else if (u == 0 && j == 1) mma_bf16_16816_zero(c1, q0, q1, q2, q3, b0, b1);
-        else if (j & 1) mma_bf16_16816(c1, q0, q1, q2, q3, b0, b1);
-        else mma_bf16_16816(c0, q0, q1, q2, q3, b0, b1);
+        if (u == 0 && j == 0) mma_bf16_16816_zero(c0, q[0], q[1], q[2], q[3], b0, b1);
+        else if (u == 0 && j == 1) mma_bf16_16816_zero(c1, q[0], q[1], q[2], q[3], b0, b1);
+        else if (j & 1) mma_bf16_16816(c1, q[0], q[1], q[2], q[3], b0, b1);
+        else mma_bf16_16816(c0, q[0], q[1], q[2], q[3], b0, b1);
       }
     }
     const uint2 sxb = lds_64(gsum_a + (uint32_t)slot_abs * 32u);
@@ -541,12 +516,7 @@ linear_w4a16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, con
     return;
   } else {
 #pragma unroll
-    for (int m = 0; m < kMT; ++m) {
-      red[warp][m][g * 8 + 2 * t] = acc[m][0];
-      red[warp][m][g * 8 + 2 * t + 1] = acc[m][1];
-      red[warp][m][(g + 8) * 8 + 2 * t] = acc[m][2];
-      red[warp][m][(g + 8) * 8 + 2 * t + 1] = acc[m][3];
-    }
+    for (int m = 0; m < kMT; ++m) store_c_frag(red[warp][m], acc[m], g, t);
     __syncthreads();
     for (int i = threadIdx.x; i < kTilesPerCta * kMT * 128; i += blockDim.x) {
       const int tl = i / (kMT * 128), rem = i % (kMT * 128);
@@ -654,12 +624,7 @@ linear_bf16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, cons
   pdl_launch_dependents();
 
 #pragma unroll
-  for (int m = 0; m < kMT; ++m) {
-    red[warp][m][g * 8 + 2 * t] = acc[m][0];
-    red[warp][m][g * 8 + 2 * t + 1] = acc[m][1];
-    red[warp][m][(g + 8) * 8 + 2 * t] = acc[m][2];
-    red[warp][m][(g + 8) * 8 + 2 * t + 1] = acc[m][3];
-  }
+  for (int m = 0; m < kMT; ++m) store_c_frag(red[warp][m], acc[m], g, t);
   __syncthreads();
   for (int i = threadIdx.x; i < kMT * 128; i += blockDim.x) {
     const int m = i >> 7, r = (i & 127) >> 3, c = i & 7;
@@ -691,8 +656,8 @@ static int w4_decode_form() {
   int f = g_w4_decode_form.load(std::memory_order_relaxed);
   if (f < 0) {
     const char* e = getenv("XB_W4_EXACT");
-    f = e ? atoi(e) : 0;            // 2 (experiment): exact form only for the big shapes (N * K >= 2^25: gate_up, down)
-    if (f < 0 || f > 2) f = 0;
+    f = e ? atoi(e) : 0;
+    if (f < 0 || f > 1) f = 0;
     g_w4_decode_form.store(f, std::memory_order_relaxed);
   }
   return f;
@@ -705,6 +670,75 @@ extern "C" int xb_set_w4_decode_form(int form) {
   const int old = w4_decode_form();
   g_w4_decode_form.store(form, std::memory_order_relaxed);
   return old;
+}
+
+// ring depth: 8 k64 tiles (4 KB) per warp in flight = 64 KB per SM at 2 CTAs/SM, ~1.5x the HBM latency-bandwidth
+// product; the ring lives in shared memory, so the depth no longer competes with the accumulators for registers
+// (a 12-tile ring measured the same as 8 tiles on every decode shape)
+static constexpr int kW4RingTiles = 8;
+
+// The kernel arguments of one W4 launch and the runtime choices of w4_small_m_impl that select its instantiation.
+struct W4Launch {
+  __nv_bfloat16* y;
+  int64_t y_stride;
+  const __nv_bfloat16* x;
+  int64_t x_stride;
+  const uint4* qw;
+  const uint32_t* meta;
+  const __nv_bfloat16* bias;
+  int M, N, K, gshift, act_mode;
+  W4Fuse fz;
+  cudaStream_t stream;
+  size_t xs_bytes;
+  int split, epi;
+  bool tg2, xs, exact;
+};
+
+template <int kMT, int kSplit, int kTG, int kEpi, bool kXs, bool kExact>
+static int w4_launch(const W4Launch& l) {
+  constexpr int kDepth = kW4RingTiles / kTG;
+  constexpr auto kern = linear_w4a16_small_m_kernel<kMT, kSplit, kDepth, kTG, 2, kEpi, kXs, kExact>;
+  // static reduction scratch + ring (+ x stage) may exceed the default 48 KB
+  XB_CUDA_OK(set_max_dynamic_smem_once<kern>((int)(w4_ring_bytes(kDepth, kTG) + (kXs ? kXsMaxBytes : 0))));
+  const dim3 grid((l.N / 16 + kWarps / kSplit - 1) / (kWarps / kSplit)), block(kWarps * 32);
+  XB_CUDA_OK(launch(kern, grid, block, w4_ring_bytes(kDepth, kTG) + l.xs_bytes, l.stream, true, l.y, l.y_stride, l.x,
+                    l.x_stride, l.qw, l.meta, l.bias, l.M, l.N, l.K, l.gshift, l.act_mode, l.fz));
+  return 0;
+}
+
+// Runtime choices -> template arguments, instantiating only the supported variants: the staged-x, exact-dequant, rope
+// and residual forms serve one token tile (M <= 8), and the residual epilogue (3) lives in the k-split reduction.
+template <int kMT, int kSplit, int kEpi, bool kXs, bool kExact>
+static int w4_pick_tg(const W4Launch& l) {
+  return l.tg2 ? w4_launch<kMT, kSplit, 2, kEpi, kXs, kExact>(l) : w4_launch<kMT, kSplit, 1, kEpi, kXs, kExact>(l);
+}
+template <int kMT, int kSplit, bool kXs, bool kExact>
+static int w4_pick_epi(const W4Launch& l) {
+  if constexpr (kMT == 1) {
+    if (l.epi == 3) {
+      if constexpr (kSplit > 1) return w4_pick_tg<1, kSplit, 3, kXs, kExact>(l);
+      return 0;   // not reached: w4_small_m_impl gives epilogue 3 a split of at least 2
+    }
+    if (l.epi == 2) return w4_pick_tg<1, kSplit, 2, kXs, kExact>(l);
+  }
+  return l.epi == 1 ? w4_pick_tg<kMT, kSplit, 1, kXs, kExact>(l) : w4_pick_tg<kMT, kSplit, 0, kXs, kExact>(l);
+}
+template <int kMT, int kSplit>
+static int w4_pick_form(const W4Launch& l) {
+  if constexpr (kMT == 1) {
+    if (l.exact) return w4_pick_epi<1, kSplit, true, true>(l);
+    if (l.xs) return w4_pick_epi<1, kSplit, true, false>(l);
+  }
+  return w4_pick_epi<kMT, kSplit, false, false>(l);
+}
+template <int kMT>
+static int w4_pick_split(const W4Launch& l) {
+  switch (l.split) {
+    case 1: return w4_pick_form<kMT, 1>(l);
+    case 2: return w4_pick_form<kMT, 2>(l);
+    case 4: return w4_pick_form<kMT, 4>(l);
+    default: return w4_pick_form<kMT, 8>(l);
+  }
 }
 
 // epi: 0 plain (+bias), 1 gate/up + activation (act_mode), 2 qkv rope + KV scatter (fz).  xs: stage x in shared memory
@@ -722,16 +756,10 @@ static int w4_small_m_impl(void* y, int64_t y_stride, const void* x, int64_t x_s
   XB_CHECK(!xs || w4_xs_bytes(M, K) <= kXsMaxBytes, "linear_w4a16_small_m: M=%d x K=%d does not fit the shared-memory x stage", M, K);
   W4Fuse fz{};
   if (fzp) fz = *fzp;
-  auto* yy = reinterpret_cast<__nv_bfloat16*>(y);
-  auto* xx = reinterpret_cast<const __nv_bfloat16*>(x);
-  auto* qw = reinterpret_cast<const uint4*>(qweight);
-  auto* bb = reinterpret_cast<const __nv_bfloat16*>(bias);
-  cudaStream_t s = (cudaStream_t)stream;
   // pick the k split so that (row tiles x splits) covers ~16 warps on each of the device's SMs
   const int ntiles = N / 16, ktiles = K / 64;
   int split = 1;
-  static const int sms = [] { int d = 0, n = 132; cudaGetDevice(&d); cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, d); return n; }();
-  while (split < 8 && ntiles * split < sms * 16 && ktiles / (split * 2) >= 3) split *= 2;
+  while (split < 8 && ntiles * split < device_sm_count() * 16 && ktiles / (split * 2) >= 3) split *= 2;
   if (epi == 3 && split < 2) split = 2;   // the residual + statistics epilogue lives in the k-split reduction
   const int tpg = group_size / 64;   // k64 tiles per quantisation group
   XB_CHECK((tpg & (tpg - 1)) == 0, "linear_w4a16_small_m: group_size/64 must be a power of two (got %d)", group_size);
@@ -739,78 +767,18 @@ static int w4_small_m_impl(void* y, int64_t y_stride, const void* x, int64_t x_s
   while ((1 << gshift) < tpg) ++gshift;
   const bool tg2 = tpg >= 2;
   // exact-dequant form: one token tile, ring slot = one group, no norm prologue, x + group sums fit the shared-memory stage
-  const int form = w4_decode_form();
-  const bool exact = (form == 1 || (form == 2 && (int64_t)N * K >= (1ll << 25))) && M <= 8 && (tpg == 1 || tpg == 2) && fz.norm_w == nullptr &&
+  const bool exact = w4_decode_form() == 1 && M <= 8 && (tpg == 1 || tpg == 2) && fz.norm_w == nullptr &&
                      w4_xs_bytes(M, K) + w4_gsum_bytes(K, group_size) <= kXsMaxBytes;
   if (exact) xs = true;
   const size_t xs_bytes = (xs ? w4_xs_bytes(M, K) : 0) + (exact ? w4_gsum_bytes(K, group_size) : 0);
-#define XB_W4_GO(MT, SP, DEPTH, TG, EPI, XS, EX)                                                                   \
-  {                                                                                                                 \
-    auto kern = linear_w4a16_small_m_kernel<MT, SP, DEPTH, TG, 2, EPI, XS, EX>;                                     \
-    static bool attr_done = false; /* per instantiation: static reduction scratch + ring may exceed 48 KB */        \
-    if (!attr_done) {                                                                                               \
-      XB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,                            \
-                                      (int)(w4_ring_bytes(DEPTH, TG) + (XS ? kXsMaxBytes : 0))));                   \
-      attr_done = true;                                                                                             \
-    }                                                                                                               \
-    XB_CUDA_OK(launch(kern, grid, block, w4_ring_bytes(DEPTH, TG) + xs_bytes, s, true, yy, y_stride, xx, x_stride,  \
-                      qw, meta, bb, M, N, K, gshift, act_mode, fz));                                                \
-  }
-#define XB_W4_TG(MT, SP, DP, EPI, XS)                                       \
-  if (tg2) { XB_W4_GO(MT, SP, (DP + 1) / 2, 2, EPI, XS, false) }            \
-  else { XB_W4_GO(MT, SP, DP, 1, EPI, XS, false) }
-#define XB_W4_EX(SP, DP, EPI)                                               \
-  if (tg2) { XB_W4_GO(1, SP, (DP + 1) / 2, 2, EPI, true, true) }            \
-  else { XB_W4_GO(1, SP, DP, 1, EPI, true, true) }
-  // the fused variants (x staged in shared memory / rope epilogue) exist for one token tile (M <= 8) only
-#define XB_W4_LAUNCH(MT, SP, DP)                                                                               \
-  {                                                                                                            \
-    dim3 grid((ntiles + (kWarps / SP) - 1) / (kWarps / SP)), block(kWarps * 32);                               \
-    if constexpr (MT == 1) {                                                                                   \
-      if (exact) {                                                                                             \
-        if (epi == 3) {                                                                                        \
-          if constexpr (SP > 1) { XB_W4_EX(SP, DP, 3) }                                                        \
-        } else if (epi == 2) { XB_W4_EX(SP, DP, 2) }                                                           \
-        else if (epi == 1) { XB_W4_EX(SP, DP, 1) }                                                             \
-        else { XB_W4_EX(SP, DP, 0) }                                                                           \
-      } else if (epi == 3) {                                                                                   \
-        if constexpr (SP > 1) {                                                                                \
-          if (xs) { XB_W4_TG(1, SP, DP, 3, true) }                                                             \
-          else { XB_W4_TG(1, SP, DP, 3, false) }                                                               \
-        }                                                                                                      \
-      } else if (xs) {                                                                                         \
-        if (epi == 2) { XB_W4_TG(1, SP, DP, 2, true) }                                                         \
-        else if (epi == 1) { XB_W4_TG(1, SP, DP, 1, true) }                                                    \
-        else { XB_W4_TG(1, SP, DP, 0, true) }                                                                  \
-      } else if (epi == 2) { XB_W4_TG(1, SP, DP, 2, false) }                                                   \
-      else if (epi == 1) { XB_W4_TG(1, SP, DP, 1, false) }                                                     \
-      else { XB_W4_TG(1, SP, DP, 0, false) }                                                                   \
-    } else {                                                                                                   \
-      if (epi == 1) { XB_W4_TG(MT, SP, DP, 1, false) }                                                         \
-      else { XB_W4_TG(MT, SP, DP, 0, false) }                                                                  \
-    }                                                                                                          \
-  }
-#define XB_W4(MT, DP)                                   \
-  switch (split) {                                      \
-    case 1: XB_W4_LAUNCH(MT, 1, DP) break;              \
-    case 2: XB_W4_LAUNCH(MT, 2, DP) break;              \
-    case 4: XB_W4_LAUNCH(MT, 4, DP) break;              \
-    default: XB_W4_LAUNCH(MT, 8, DP) break;             \
-  }
   XB_CHECK(!(epi == 1 && M > 16), "linear_w4a16_gate_up_act_small_m: M=%d > 16, use the GEMM + act_and_mul_interleaved8", M);
-  // ring depth: 8 k64 tiles (4 KB) per warp in flight = 64 KB per SM at 2 CTAs/SM, ~1.5x the HBM latency-bandwidth
-  // product; the ring lives in shared memory, so the depth no longer competes with the accumulators for registers
-  // (a 12-tile ring measured the same as 8 tiles on every decode shape)
-  if (M <= 8) { XB_W4(1, 8) }
-  else if (M <= 16) { XB_W4(2, 8) }
-  else if (M <= 32) { XB_W4(4, 8) }
-  else { XB_W4(8, 8) }
-#undef XB_W4_GO
-#undef XB_W4_TG
-#undef XB_W4_EX
-#undef XB_W4_LAUNCH
-#undef XB_W4
-  return 0;
+  const W4Launch l{reinterpret_cast<__nv_bfloat16*>(y), y_stride, reinterpret_cast<const __nv_bfloat16*>(x), x_stride,
+                   reinterpret_cast<const uint4*>(qweight), meta, reinterpret_cast<const __nv_bfloat16*>(bias),
+                   M, N, K, gshift, act_mode, fz, (cudaStream_t)stream, xs_bytes, split, epi, tg2, xs, exact};
+  if (M <= 8) return w4_pick_split<1>(l);
+  if (M <= 16) return w4_pick_split<2>(l);
+  if (M <= 32) return w4_pick_split<4>(l);
+  return w4_pick_split<8>(l);
 }
 
 extern "C" int xb_linear_w4a16_small_m(void* y, int64_t y_stride, const void* x, int64_t x_stride,

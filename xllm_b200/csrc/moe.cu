@@ -214,20 +214,10 @@ moe_expert_gemv_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, const __
 
 // ---------------------------------------------------------------------------------------------------------------------
 // W4A16 experts (SURVEY cfg[4] "MoE W4A16"; additive like the dense W4A16 linears - the reference's CUDA FusedMoE takes
-// unquantised experts only): the same expert-indexed GEMV over the tile-packed int4 layout of linear_small_m.cu, per expert
-//   qweight [E][rows/16][K/64][32 lanes][4] u32,  meta [E][K/g][rows] u32 (bf16 scale | bf16(128 + zero) << 16),
-// dequantised bit-exactly as w = bf16((q - z) * s) (spec form 1 of oracle/quant.py) right before the mma.
+// unquantised experts only): the same expert-indexed GEMV over the tile-packed int4 layout of linear_small_m.cu, one
+// [rows/16][K/64][32][4] weight and one [K/g][rows] meta block per expert, dequantised by w4_dequant_word (common.cuh)
+// right before the mma.
 // ---------------------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t moe_lop3_and_or(uint32_t a, uint32_t mask, uint32_t orv) {
-  uint32_t d;
-  asm("lop3.b32 %0, %1, %2, %3, 0xea;" : "=r"(d) : "r"(a), "r"(mask), "r"(orv));
-  return d;
-}
-__device__ __forceinline__ uint32_t moe_hsub2(uint32_t a, uint32_t b) {
-  uint32_t d;
-  asm("sub.rn.bf16x2 %0, %1, %2;" : "=r"(d) : "r"(a), "r"(b));
-  return d;
-}
 
 template <bool kSwiGLU>
 __global__ void __launch_bounds__(256)
@@ -289,18 +279,16 @@ moe_expert_gemv_w4_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, const
           }
 #pragma unroll
           for (int h = 0; h < kH; ++h) {
-            const uint32_t s0 = __byte_perm(m0[h][u], 0, 0x1010), z0 = __byte_perm(m0[h][u], 0, 0x3232);
-            const uint32_t s1 = __byte_perm(m1[h][u], 0, 0x1010), z1 = __byte_perm(m1[h][u], 0, 0x3232);
+            uint32_t s0, z0, s1, z1;
+            w4_meta(m0[h][u], s0, z0);
+            w4_meta(m1[h][u], s1, z1);
             const uint32_t* wv = &wq[h][u].x;
 #pragma unroll
             for (int j = 0; j < 4; ++j) {
-              const uint32_t w = wv[j];
-              const uint32_t a0 = hmul2_bf16x2(moe_hsub2(moe_lop3_and_or(w, 0x000f000fu, 0x43004300u), z0), s0);
-              const uint32_t a1 = hmul2_bf16x2(moe_hsub2(moe_lop3_and_or(w >> 4, 0x000f000fu, 0x43004300u), z1), s1);
-              const uint32_t a2 = hmul2_bf16x2(moe_hsub2(moe_lop3_and_or(w >> 8, 0x000f000fu, 0x43004300u), z0), s0);
-              const uint32_t a3 = hmul2_bf16x2(moe_hsub2(moe_lop3_and_or(w >> 12, 0x000f000fu, 0x43004300u), z1), s1);
+              uint32_t a[4];
+              w4_dequant_word(wv[j], z0, s0, z1, s1, a);
               const uint32_t* xv = j < 2 ? &xlo.x : &xhi.x;
-              mma_bf16_16816(acc[h], a0, a1, a2, a3, xv[(j & 1) * 2], xv[(j & 1) * 2 + 1]);
+              mma_bf16_16816(acc[h], a[0], a[1], a[2], a[3], xv[(j & 1) * 2], xv[(j & 1) * 2 + 1]);
             }
           }
         }

@@ -555,14 +555,14 @@ unsigned long long* g_decode_trace = nullptr;   // debug only (xb_debug_set_deco
 template <int kD, int kGT, int kW>
 static int launch_decode_w(DecodeParams& p, int batch, int splits, cudaStream_t stream) {
   constexpr int kHeads = 8 * kGT;
-  const size_t smem = ((size_t)kW * kHeads * (kD + 4 + 2) + (size_t)kHeads * (kD + 1) + 3) * sizeof(float);
-  auto kern = paged_decode_kernel<kD, kGT, kW>;
-  static bool attr_done = false;  // per instantiation
-  static int max_cluster = 1;     // largest cluster size this device can co-schedule for this kernel
-  if (!attr_done) {
-    XB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  constexpr size_t smem = ((size_t)kW * kHeads * (kD + 4 + 2) + (size_t)kHeads * (kD + 1) + 3) * sizeof(float);
+  constexpr auto kern = paged_decode_kernel<kD, kGT, kW>;
+  XB_CUDA_OK(set_max_dynamic_smem_once<kern>((int)smem));
+  // largest cluster size this device can co-schedule for this kernel (probed once per instantiation)
+  static const int max_cluster = [] {
     // clusters of more than 8 CTAs are "non-portable": allowed explicitly, then verified with an occupancy query
     cudaFuncSetAttribute(kern, cudaFuncAttributeNonPortableClusterSizeAllowed, 1);
+    int max_c = 1;
     for (int c : {16, 8, 4, 2}) {
       cudaLaunchConfig_t cfg{};
       cfg.gridDim = dim3(c, 1, 1);
@@ -577,13 +577,13 @@ static int launch_decode_w(DecodeParams& p, int batch, int splits, cudaStream_t 
       cfg.numAttrs = 1;
       int n = 0;
       if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) == cudaSuccess && n > 0) {
-        max_cluster = c;
+        max_c = c;
         break;
       }
     }
     cudaGetLastError();   // a failed probe must not poison the next launch's error state
-    attr_done = true;
-  }
+    return max_c;
+  }();
   // the plan's cluster size is a request: fall back to per-CTA partials (cluster 1) when the device cannot co-schedule it
   if (p.cluster > max_cluster || splits % p.cluster != 0) p.cluster = 1;
   p.trace = g_decode_trace;

@@ -316,12 +316,8 @@ template <int kD>
 static int launch_prefill(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const PrefillParams& p,
                           int batch, int q_tiles, cudaStream_t stream) {
   using Cfg = PrefillCfg<kD>;
-  auto kern = prefill_attention_kernel<kD>;
-  static bool attr_done = false;
-  if (!attr_done) {
-    XB_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::kSmemBytes));
-    attr_done = true;
-  }
+  constexpr auto kern = prefill_attention_kernel<kD>;
+  XB_CUDA_OK(set_max_dynamic_smem_once<kern>(Cfg::kSmemBytes));
   dim3 grid(q_tiles, p.num_kv_heads, batch * p.kv_splits), block(kPrefillThreads);
   XB_CUDA_OK(launch(kern, grid, block, (size_t)Cfg::kSmemBytes, stream, true, tq, tk, tv, p));
   if (p.kv_splits > 1)
