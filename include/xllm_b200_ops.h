@@ -394,7 +394,7 @@ int xb_embedding_bf16(void* out, const int32_t* token_ids, const void* table,
 int xb_argmax_bf16(int32_t* out, const void* logits, int64_t stride, int rows,
                    int vocab, xb_stream_t stream);
 
-/* ---- Mixture of experts, decode-sized token counts (SURVEY 8f n4) ---------------------------------------------------------
+/* ---- Mixture of experts (SURVEY 8f n4) ------------------------------------------------------------------------------------
  * xb_moe_fused_topk replaces xllm::kernel::cuda::moe_fused_topk (cuda_ops_api.h:251-256, moe/moe_fused_topk.cu:22-58):
  *   gating_output [T, E] fp32 or bf16 (row stride in elements), scoring softmax (scoring_sigmoid = 0) or sigmoid with an
  *   optional fp32 correction bias [E] (added for the selection, subtracted from the returned weight), top-k with ties to the
@@ -403,12 +403,28 @@ int xb_argmax_bf16(int32_t* out, const void* logits, int64_t stride, int rows,
  * xb_moe_experts_bf16 replaces xllm::kernel::cuda::cutlass_fused_moe (cuda_ops_api.h:260-289, moe/fused_moe.cpp:23-124) for
  *   unquantised bf16 experts (all the reference's CUDA FusedMoE accepts, layers/cuda/fused_moe.cpp:39-42): fc1 [E_local, 2I, H]
  *   in [up | gate] row order, fc2 [E_local, H, I]; out[t] = bf16(sum_k scale[t,k] * bf16(fc2_e . bf16(silu(gate) * up))).
- *   Experts outside [expert_begin, expert_begin + num_local_experts) contribute zero (expert parallelism: the caller
- *   all-reduces, layers/cuda/fused_moe.cpp:116-117).  workspace: xb_moe_experts_workspace_bytes. */
+ *   Experts outside [expert_begin, expert_begin + num_local_experts) contribute zero, whatever the id, negative ids included
+ *   (expert parallelism: the caller all-reduces, layers/cuda/fused_moe.cpp:116-117).
+ * The expert entries take one of two paths by the token count T alone (P = T * topk pairs):
+ *   T <= 64 (decode): one expert-indexed GEMV per pair, each streaming its expert's weights; P <= 65535.
+ *   T >= 65 (prefill): the local pairs are sorted by expert on the device (stable), their input rows gathered, and two grouped
+ *     wgmma GEMMs over the stacked expert weights run fc1 + SwiGLU and fc2, tensor-core bound; T <= 65535, topk <= 32,
+ *     num_local_experts <= 512.  No host synchronisation: one captured CUDA graph replays with any routing.
+ * workspace: xb_moe_experts_workspace_bytes(T, topk, H, I) bytes, 16-byte aligned, scratch only (no state between calls):
+ *   T <= 64:  P * (I + H) * 2                                         (act, y2)
+ *   T >= 65:  8192 + 2 * round_up(4 * P, 256) + P * (2H + I) * 2     (routing header for up to 512 experts, row_of_pair and
+ *             pair_of_row maps, the expert-sorted input rows, act, y2)
+ * xb_moe_experts_describe (host-only, no device): the path the entries take for a shape, as text ("bf16 gemv",
+ *   "w4 grouped bn=128 m_tiles<=40"); kind 0 bf16 | 2 w4a16 (the codes of xb_gemm_describe).  Returns the length, -1 on a bad
+ *   kind.  xb_set_moe_grouped_min_tokens: the smallest T that takes the grouped path (>= 1; default 65, env
+ *   XB_MOE_GROUPED_MIN_TOKENS), for tests and sweeps; returns the old value, -1 on a bad value. */
 int xb_moe_fused_topk(float* topk_weights, int32_t* topk_ids, const void* gating_output, int gating_is_bf16,
                       int64_t gating_stride, const float* correction_bias, int num_tokens, int num_experts, int topk,
                       int renormalize, int scoring_sigmoid, xb_stream_t stream);
 int64_t xb_moe_experts_workspace_bytes(int num_tokens, int topk, int hidden, int inter);
+int xb_moe_experts_describe(int kind, int num_tokens, int topk, int hidden, int inter, int num_local_experts, char* buf,
+                            int buf_len);
+int xb_set_moe_grouped_min_tokens(int min_tokens);
 int xb_moe_experts_bf16(void* out, int64_t out_stride, const void* input, int64_t in_stride,
                         const int32_t* token_selected_experts, const float* token_final_scales,
                         const void* fc1_weights, const void* fc2_weights, int num_tokens, int topk, int hidden,
@@ -417,8 +433,8 @@ int xb_moe_experts_bf16(void* out, int64_t out_stride, const void* input, int64_
 
 /* W4A16 experts (BASELINE configs[4] "MoE W4A16"; additive like the dense weight-only linears): per expert the tile-packed
  * int4 layout of xb_linear_w4a16_small_m - fc1 qweight [E_local, 2I/16, H/64, 32, 4] u32 + meta [E_local, H/g, 2I] u32 (rows
- * [up | gate]), fc2 qweight [E_local, H/16, I/64, 32, 4] + meta [E_local, I/g, H]; same arithmetic as xb_moe_experts_bf16 on
- * the dequantised weights w = bf16((q - z) * s). */
+ * [up | gate]), fc2 qweight [E_local, H/16, I/64, 32, 4] + meta [E_local, I/g, H]; same arithmetic and the same two paths as
+ * xb_moe_experts_bf16 on the dequantised weights w = bf16((q - z) * s).  The grouped path also needs 16-byte aligned meta. */
 int xb_moe_experts_w4a16(void* out, int64_t out_stride, const void* input, int64_t in_stride,
                          const int32_t* token_selected_experts, const float* token_final_scales,
                          const uint32_t* fc1_qweight, const uint32_t* fc1_meta, const uint32_t* fc2_qweight,

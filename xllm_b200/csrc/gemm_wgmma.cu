@@ -105,7 +105,21 @@ struct GemmParams {
   int split_k;
   float* splitk_ws;            // [tiles][split_k][kBlockN][128] fp32
   unsigned int* splitk_tickets;  // [tiles], zero at rest
+  // grouped MoE experts (kGroup != 0, the prefill path of moe.cu): A is the expert-sorted activation buffer [M = pairs, K],
+  // B the local experts' weights stacked along N.  The tile count and every tile's expert come from the routing header the
+  // route kernel wrote on the device (no host read).  fc1 (kGroupFc1): a tile loads up rows n0.. and gate rows I + n0.. as
+  // two half boxes and the epilogue writes c[row][n0 + c] = bf16(silu(gate) * up) from the fp32 sums; fc2 (kGroupFc2): the
+  // epilogue stores sorted row r to c[pair_of_row[r]], back in pair order.  N is I (fc1) or H (fc2).
+  const int* grp_row_start;    // [E + 1] first sorted row of each local expert
+  const int* grp_mtile_start;  // [E + 1] first 128-row m tile of each local expert
+  const int* grp_pair_of_row;  // fc2: the pair (y2 row) of each sorted row
+  int grp_experts;
+  int grp_b_rows;              // weight rows per expert: 2I (fc1) or H (fc2)
+  int grp_half;                // fc1: offset of the gate rows (I)
+  int grp_meta_rows;           // W4: meta rows per expert (K / group_size)
 };
+
+enum { kGroupNone = 0, kGroupFc1 = 1, kGroupFc2 = 2 };
 
 constexpr int kBlockM = 128;
 constexpr int kConsumerWGs = 2;                 // 64 rows each
@@ -159,12 +173,41 @@ __device__ __forceinline__ void e4m3x4_to_f16(uint32_t w, uint32_t& lo, uint32_t
       : "=r"(lo), "=r"(hi) : "r"(w));
 }
 
-template <int kKind, int kBlockN>
+// grouped mode: linear tile index -> (local expert, m block within the expert, n block).  Expert e owns the tiles
+// [mtile_start[e] * n_blocks, mtile_start[e + 1] * n_blocks), m fastest, so the m blocks of one expert run next to each other
+// and share every B tile through L2.  Experts without rows own no tiles.
+struct GroupTile {
+  int e, m_blk, n_blk;
+  int a_row;   // first sorted row of the tile
+  int rows;    // rows of the tile that belong to expert e (the rest are the next expert's or past the end: masked)
+};
+__device__ __forceinline__ GroupTile group_tile(const GemmParams& p, int tile, int n_blocks) {
+  const int* ms = p.grp_mtile_start;
+  int lo = 0, hi = p.grp_experts;   // ms[lo] * n_blocks <= tile < ms[hi] * n_blocks
+  while (hi - lo > 1) {
+    const int mid = (lo + hi) >> 1;
+    if (ms[mid] * n_blocks <= tile) lo = mid;
+    else hi = mid;
+  }
+  GroupTile g;
+  const int mt = ms[lo + 1] - ms[lo];
+  const int local = tile - ms[lo] * n_blocks;
+  g.e = lo;
+  g.n_blk = local / mt;
+  g.m_blk = local - g.n_blk * mt;
+  g.a_row = p.grp_row_start[lo] + g.m_blk * kBlockM;
+  g.rows = min(kBlockM, p.grp_row_start[lo + 1] - g.a_row);
+  return g;
+}
+
+template <int kKind, int kBlockN, int kGroup = kGroupNone>
 __global__ void __launch_bounds__(GemmCfg<kKind, kBlockN>::kThreads, 1)
 gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b,
                   const __grid_constant__ CUtensorMap tmap_m, const GemmParams p) {
   using Cfg = GemmCfg<kKind, kBlockN>;
   constexpr int kStages = Cfg::kStages;
+  static_assert(kGroup == kGroupNone || kKind == kKindBF16 || kKind == kKindW4, "grouped mode: bf16 and W4 only");
+  constexpr int kTileCols = kGroup == kGroupFc1 ? kBlockN / 2 : kBlockN;   // output columns of a tile (fc1: up | gate halves)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* bbuf = smem + kStages * Cfg::kStageBytes;                  // [kBStages][kRingBytes] converted operand ring
@@ -178,13 +221,13 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_blocks = (p.M + kBlockM - 1) / kBlockM;
-  const int n_blocks = (p.N + kBlockN - 1) / kBlockN;
+  const int n_blocks = (p.N + kTileCols - 1) / kTileCols;
   const int num_kb = (p.K + Cfg::kBlockK - 1) / Cfg::kBlockK;
   // split-K exists in the swap-AB FP8 instantiations only (compile-time off elsewhere)
   constexpr bool kSplitOK = kKind == kKindFP8 && kBlockN <= 64;
   const int split_k = kSplitOK ? p.split_k : 1;
   const int kb_per = (num_kb + split_k - 1) / split_k;
-  const int num_tiles = m_blocks * n_blocks * split_k;      // work units: (output tile, k range); the splits of a tile are adjacent
+  int num_tiles = m_blocks * n_blocks * split_k;      // work units: (output tile, k range); the splits of a tile are adjacent
 
   auto stage_a = [&](int s) { return smem + s * Cfg::kStageBytes; };
   auto stage_b = [&](int s) { return smem + s * Cfg::kStageBytes + Cfg::kABytes; };               // BF16
@@ -214,6 +257,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 
   pdl_launch_dependents();
   pdl_wait();   // A (activations) comes from the producer kernel
+  if constexpr (kGroup != kGroupNone) num_tiles = p.grp_mtile_start[p.grp_experts] * n_blocks;   // written by the route kernel
 
   if (warp == 0) {
     // ======================= TMA producer =======================
@@ -224,6 +268,15 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
         const int otile = tile / split_k, ks = tile - otile * split_k;
         const int m_blk = otile % m_blocks, n_blk = otile / m_blocks;
         const int kb0 = ks * kb_per, kb1 = min(num_kb, kb0 + kb_per);
+        // first A row, first B (weight) row and first meta row / column of the tile; grouped: offset to the tile's expert
+        int a_row = m_blk * kBlockM, b_row = n_blk * kBlockN, meta_row = 0, meta_col = n_blk * kBlockN;
+        if constexpr (kGroup != kGroupNone) {
+          const GroupTile gt = group_tile(p, tile, n_blocks);
+          a_row = gt.a_row;
+          b_row = gt.e * p.grp_b_rows + gt.n_blk * kTileCols;
+          meta_row = gt.e * p.grp_meta_rows;
+          meta_col = gt.n_blk * kTileCols;
+        }
         for (int kb = kb0; kb < kb1; ++kb) {
           mbar_wait(empty_bar + s, ph ^ 1);
           if (kind_is_wq(kKind)) {
@@ -231,18 +284,25 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
             // box [kBlockN/16][128 words], no swizzle), plus the group's scale/zero words for these rows (tensor [K/g][N])
             mbar_expect_tx(packed_bar + s, Cfg::kPackedBytes + Cfg::kMetaBytes);
             // (W8: one byte per weight - 256 words per row tile and k tile instead of 128)
-            tma_load_2d(stage_packed(s), &tmap_b, packed_bar + s, kb * (kKind == kKindW8 ? 256 : 128), n_blk * kBlockN / 16);
-            tma_load_2d(stage_meta(s), &tmap_m, packed_bar + s, n_blk * kBlockN, kb >> p.gshift);
+            tma_load_2d(stage_packed(s), &tmap_b, packed_bar + s, kb * (kKind == kKindW8 ? 256 : 128), b_row / 16);
+            tma_load_2d(stage_meta(s), &tmap_m, packed_bar + s, meta_col, meta_row + (kb >> p.gshift));
+            if constexpr (kGroup == kGroupFc1) {   // the matching gate rows: second half of the packed tile and of the meta
+              tma_load_2d(stage_packed(s) + Cfg::kPackedBytes / 2, &tmap_b, packed_bar + s, kb * 128, (b_row + p.grp_half) / 16);
+              tma_load_2d(stage_meta(s) + Cfg::kMetaBytes / 2, &tmap_m, packed_bar + s, meta_col + p.grp_half,
+                          meta_row + (kb >> p.gshift));
+            }
             mbar_expect_tx(full_bar + s, Cfg::kABytes);
-            tma_load_2d(stage_a(s), &tmap_a, full_bar + s, kb * Cfg::kBlockK, m_blk * kBlockM);
+            tma_load_2d(stage_a(s), &tmap_a, full_bar + s, kb * Cfg::kBlockK, a_row);
           } else if (kKind == kKindFP8) {
             mbar_expect_tx(full_bar + s, Cfg::kABytes + Cfg::kPackedBytes);
-            tma_load_2d(stage_a(s), &tmap_a, full_bar + s, kb * Cfg::kBlockK, m_blk * kBlockM);
-            tma_load_2d(stage_packed(s), &tmap_b, full_bar + s, kb * Cfg::kBlockK, n_blk * kBlockN);
+            tma_load_2d(stage_a(s), &tmap_a, full_bar + s, kb * Cfg::kBlockK, a_row);
+            tma_load_2d(stage_packed(s), &tmap_b, full_bar + s, kb * Cfg::kBlockK, b_row);
           } else {
             mbar_expect_tx(full_bar + s, Cfg::kABytes + Cfg::kBBytes);
-            tma_load_2d(stage_a(s), &tmap_a, full_bar + s, kb * Cfg::kBlockK, m_blk * kBlockM);
-            tma_load_2d(stage_b(s), &tmap_b, full_bar + s, kb * Cfg::kBlockK, n_blk * kBlockN);
+            tma_load_2d(stage_a(s), &tmap_a, full_bar + s, kb * Cfg::kBlockK, a_row);
+            tma_load_2d(stage_b(s), &tmap_b, full_bar + s, kb * Cfg::kBlockK, b_row);
+            if constexpr (kGroup == kGroupFc1)      // gate rows into the second half of the B tile
+              tma_load_2d(stage_b(s) + Cfg::kBBytes / 2, &tmap_b, full_bar + s, kb * Cfg::kBlockK, b_row + p.grp_half);
           }
           if (++s == kStages) { s = 0; ph ^= 1; }
         }
@@ -291,6 +351,41 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
       // ---- epilogue: fragment element d[4j + 2h + e] is (row r0 + 8h, column c0 + 8j + e) of the tile ----
       const int r_loc = wg * 64 + wq * 16 + (lane >> 2);
       const int c_loc = 2 * (lane & 3);
+      if constexpr (kGroup != kGroupNone) {
+        // rows past the expert's segment are masked; N (I or H) is a multiple of 32, so a column pair is in or out together
+        const GroupTile gt = group_tile(p, tile, n_blocks);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int rr = r_loc + 8 * h;
+          if (rr >= gt.rows) continue;
+          const int row = gt.a_row + rr;
+          if constexpr (kGroup == kGroupFc1) {
+            // up column c is fragment column group j < kBlockN / 16, its gate column c + kBlockN / 2 is group j + kBlockN / 16
+            __nv_bfloat16* crow = p.c + (int64_t)row * p.ldc;
+#pragma unroll
+            for (int j = 0; j < Cfg::kAcc / 8; ++j) {
+              const int col = gt.n_blk * kTileCols + 8 * j + c_loc;
+              if (col >= p.N) continue;
+              float o[2];
+#pragma unroll
+              for (int e = 0; e < 2; ++e) {
+                const float up = acc[4 * j + 2 * h + e], gate = acc[4 * (j + Cfg::kAcc / 8) + 2 * h + e];
+                o[e] = (gate / (1.0f + expf(-gate))) * up;     // silu(gate) * up on the fp32 sums, as the GEMV path
+              }
+              *reinterpret_cast<uint32_t*>(crow + col) = pack_bf16x2(o[0], o[1]);
+            }
+          } else {
+            __nv_bfloat16* crow = p.c + (int64_t)p.grp_pair_of_row[row] * p.ldc;   // back to pair order
+#pragma unroll
+            for (int j = 0; j < Cfg::kAcc / 4; ++j) {
+              const int col = gt.n_blk * kBlockN + 8 * j + c_loc;
+              if (col >= p.N) continue;
+              *reinterpret_cast<uint32_t*>(crow + col) = pack_bf16x2(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1]);
+            }
+          }
+        }
+        continue;
+      }
       if (kSplitOK && split_k > 1) {
         // leave this k range's fp32 partial in the workspace ([split][column][row]), take a ticket; the last arriver sums
         // the partials in split order (the same order whichever CTA arrived last: bit-reproducible)
@@ -467,18 +562,64 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
   }
 }
 
-template <int kKind, int kBlockN>
+template <int kKind, int kBlockN, int kGroup = kGroupNone>
 static int launch_gemm(const CUtensorMap& ta, const CUtensorMap& tb, GemmParams p, cudaStream_t stream,
                        const CUtensorMap* tm = nullptr) {
   using Cfg = GemmCfg<kKind, kBlockN>;
-  constexpr auto kern = gemm_wgmma_kernel<kKind, kBlockN>;
+  constexpr auto kern = gemm_wgmma_kernel<kKind, kBlockN, kGroup>;
   XB_CUDA_OK(set_max_dynamic_smem_once<kern>(Cfg::kSmemBytes));
   const int max_ctas = device_sm_count();     // persistent CTAs: one per SM
   if (p.split_k < 1) p.split_k = 1;
-  const int units = ((p.M + kBlockM - 1) / kBlockM) * ((p.N + kBlockN - 1) / kBlockN) * p.split_k;
-  dim3 grid(units < max_ctas ? units : max_ctas), block(Cfg::kThreads);
+  // grouped: the tile count is only known on the device; every expert adds at most one partial m tile
+  constexpr int kTileCols = kGroup == kGroupFc1 ? kBlockN / 2 : kBlockN;
+  const int64_t m_units = (p.M + kBlockM - 1) / kBlockM + (kGroup != kGroupNone ? p.grp_experts : 0);
+  const int64_t units = m_units * ((p.N + kTileCols - 1) / kTileCols) * p.split_k;
+  dim3 grid(units < max_ctas ? (unsigned)units : (unsigned)max_ctas), block(Cfg::kThreads);
   XB_CUDA_OK(launch(kern, grid, block, (size_t)Cfg::kSmemBytes, stream, true, ta, tb, tm ? *tm : ta, p));
   return 0;
+}
+
+// grouped expert GEMMs of the MoE prefill path (declared in tc_common.cuh, called by moe.cu after the routing kernels).  Shapes
+// and alignment are validated by the MoE entry points.
+//   fc1: c = act [P, I],  act[r] = bf16(silu(a[r] . gate_e) * (a[r] . up_e)),  a [P, H];  b = fc1 stacked [E * 2I, H]
+//   fc2: c = y2 [P, H],   y2[pair_of_row[r]] = bf16(a[r] . fc2_e),              a = act [P, I];  b = fc2 stacked [E * H, I]
+// W4: b is the stacked tile-packed qweight [E * rows / 16, K / 64 * 128] u32 and meta the stacked [E * K / g, rows] words.
+// BLOCK_N is 128 throughout: fc1 tiles then cover 64 output columns (64 up + 64 gate rows of B).
+int moe_grouped_gemm(int w4, int fc2, void* c, const void* a, const void* b, const uint32_t* meta, int gshift, int group_size,
+                     const int* row_start, const int* mtile_start, const int* pair_of_row, int P, int H, int I, int E,
+                     cudaStream_t stream) {
+  constexpr int kBN = 128;
+  const int N = fc2 ? H : I, K = fc2 ? I : H;
+  const int rows = fc2 ? H : 2 * I;             // weight rows per expert
+  const uint32_t box_rows = fc2 ? kBN : kBN / 2;
+  GemmParams p{};
+  p.c = reinterpret_cast<__nv_bfloat16*>(c);
+  p.ldc = N;
+  p.M = P; p.N = N; p.K = K;
+  p.gshift = gshift;
+  p.grp_row_start = row_start;
+  p.grp_mtile_start = mtile_start;
+  p.grp_pair_of_row = pair_of_row;
+  p.grp_experts = E;
+  p.grp_b_rows = rows;
+  p.grp_half = I;
+  p.grp_meta_rows = w4 ? K / group_size : 0;
+  CUtensorMap ta, tb, tm;
+  if (make_tmap_2d(&ta, a, P, K, (uint64_t)K * 2, kBlockM, 64, 2)) return 1;
+  if (!w4) {
+    if (make_tmap_2d(&tb, b, (uint64_t)E * rows, K, (uint64_t)K * 2, box_rows, 64, 2)) return 1;
+    return fc2 ? launch_gemm<kKindBF16, kBN, kGroupFc2>(ta, tb, p, stream)
+               : launch_gemm<kKindBF16, kBN, kGroupFc1>(ta, tb, p, stream);
+  }
+  const uint64_t ktiles = K / 64;
+  if (make_tmap_2d_raw(&tb, b, CU_TENSOR_MAP_DATA_TYPE_UINT32, (uint64_t)E * rows / 16, ktiles * 128, ktiles * 512, box_rows / 16,
+                       128, CU_TENSOR_MAP_SWIZZLE_NONE))
+    return 1;
+  if (make_tmap_2d_raw(&tm, meta, CU_TENSOR_MAP_DATA_TYPE_UINT32, (uint64_t)E * (K / group_size), rows, (uint64_t)rows * 4, 1,
+                       box_rows, CU_TENSOR_MAP_SWIZZLE_NONE))
+    return 1;
+  return fc2 ? launch_gemm<kKindW4, kBN, kGroupFc2>(ta, tb, p, stream, &tm)
+             : launch_gemm<kKindW4, kBN, kGroupFc1>(ta, tb, p, stream, &tm);
 }
 
 }  // namespace tc

@@ -32,6 +32,18 @@ void fused_qk_norm_rope(torch::Tensor& qkv, int64_t num_heads_q, int64_t num_hea
 std::tuple<torch::Tensor, torch::Tensor> moe_fused_topk(torch::Tensor& gating_output, int64_t topk, bool renormalize,
                                                         const std::optional<torch::Tensor>& correction_bias,
                                                         const std::string& scoring_func);
+enum class ActivationType : int8_t { GELU = 0, RELU = 1, SILU = 2, SWIGLU = 3, GEGLU = 4, SWIGLU_BIAS = 5, RELU2 = 6, IDENTITY = 7, INVALID_TYPE = 8 };
+torch::Tensor cutlass_fused_moe(const torch::Tensor& input, const torch::Tensor& token_selected_experts,
+                                const torch::Tensor& token_final_scales, const torch::Tensor& fc1_expert_weights,
+                                const torch::Tensor& fc2_expert_weights, torch::ScalarType output_dtype,
+                                const std::vector<torch::Tensor>& quant_scales, int32_t tp_size, int32_t tp_rank, int32_t ep_size,
+                                int32_t ep_rank, int32_t cluster_size, int32_t cluster_rank,
+                                const std::optional<torch::Tensor>& fc1_expert_biases, const std::optional<torch::Tensor>& fc2_expert_biases,
+                                const std::optional<torch::Tensor>& input_sf, const std::optional<torch::Tensor>& swiglu_alpha,
+                                const std::optional<torch::Tensor>& swiglu_beta, const std::optional<torch::Tensor>& swiglu_limit,
+                                const std::optional<torch::Tensor>& output, bool enable_alltoall, bool use_deepseek_fp8_block_scale,
+                                bool use_w4_group_scaling, bool use_mxfp8_act_scaling, bool min_latency_mode, bool use_packed_weights,
+                                int32_t tune_max_num_tokens, ActivationType activation_type);
 }  // namespace xllm::kernel::cuda
 
 namespace xk = xllm::kernel::cuda;
@@ -67,4 +79,13 @@ PYBIND11_MODULE(xllm_b200_shim_py, m) {
   });
   m.def("moe_fused_topk", [](torch::Tensor gating, int64_t topk, bool renormalize, std::optional<torch::Tensor> bias,
                              const std::string& scoring) { return xk::moe_fused_topk(gating, topk, renormalize, bias, scoring); });
+  // the arguments layers/cuda/fused_moe.cpp:97-115 passes: bf16 experts, no quantisation, SwiGLU, the caller reduces over TP / EP
+  m.def("cutlass_fused_moe", [](torch::Tensor input, torch::Tensor ids, torch::Tensor scales, torch::Tensor fc1, torch::Tensor fc2,
+                                int64_t ep_size, int64_t ep_rank) {
+    return xk::cutlass_fused_moe(input, ids, scales, fc1, fc2, torch::kBFloat16, {}, 1, 0, (int32_t)ep_size, (int32_t)ep_rank, 1, 0,
+                                 std::nullopt, std::nullopt, std::nullopt, std::nullopt, std::nullopt, std::nullopt, std::nullopt,
+                                 false, false, false, false, false, false, 0, xk::ActivationType::SWIGLU);
+  }, pybind11::arg("input"), pybind11::arg("token_selected_experts"), pybind11::arg("token_final_scales"),
+     pybind11::arg("fc1_expert_weights"), pybind11::arg("fc2_expert_weights"), pybind11::arg("ep_size") = 1,
+     pybind11::arg("ep_rank") = 0);
 }

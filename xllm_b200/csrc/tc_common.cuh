@@ -205,6 +205,12 @@ int make_tmap_2d_raw(CUtensorMap* out, const void* base, int dtype /*CUtensorMap
 // 3-D bf16 tensor [d2][d1][d0] (d0 contiguous), byte strides for d1 and d2, box [b2][b1][b0], 128-byte swizzle.
 int make_tmap_3d_bf16(CUtensorMap* out, const void* base, uint64_t d0, uint64_t d1, uint64_t d2, uint64_t stride1_bytes,
                       uint64_t stride2_bytes, uint32_t b0, uint32_t b1, uint32_t b2);
+// grouped expert GEMMs of the MoE prefill path (gemm_wgmma.cu): fc2 = 0 runs fc1 + SwiGLU into act [P, I], fc2 = 1 runs fc2 and
+// scatters the rows to y2 [P, H] in pair order; w4 selects the tile-packed int4 weights (meta, gshift, group_size) over bf16.
+// row_start / mtile_start / pair_of_row are the device-side routing of moe.cu.
+int moe_grouped_gemm(int w4, int fc2, void* c, const void* a, const void* b, const uint32_t* meta, int gshift, int group_size,
+                     const int* row_start, const int* mtile_start, const int* pair_of_row, int P, int H, int I, int E,
+                     cudaStream_t stream);
 
 }  // namespace tc
 }  // namespace xb

@@ -1,7 +1,7 @@
-"""FusedMoE layer composition for decode-sized batches (SURVEY 8f n4), mirroring xllm::layer::FusedMoEImpl on CUDA
+"""FusedMoE layer composition (SURVEY 8f n4), mirroring xllm::layer::FusedMoEImpl on CUDA
 (xllm/core/layers/cuda/fused_moe.cpp:28-117): replicated gate linear -> moe_fused_topk -> gated experts (bf16, unquantised:
 all the reference's CUDA FusedMoE accepts, :39-42) -> all-reduce over the MoE-TP group, then over the MoE-EP group
-(:116-117).  Weights: w13 [E_local, 2 * I_local, H] in [up | gate] order (load_experts, :124-126), w2 [E_local, H, I_local];
+(:116-117).  Any token count: decode batches run the expert GEMVs, prefill steps the grouped GEMMs (ops.cutlass_fused_moe).  Weights: w13 [E_local, 2 * I_local, H] in [up | gate] order (load_experts, :124-126), w2 [E_local, H, I_local];
 expert e of the model lives on EP rank e // E_local; the intermediate dimension is split over the TP group."""
 from typing import Optional
 

@@ -649,10 +649,30 @@ def moe_fused_topk(gating_output, topk: int, renormalize: bool, correction_bias=
     return w, ids
 
 
+def set_moe_grouped_min_tokens(min_tokens: int) -> int:
+    """smallest token count for which the MoE expert entries take the grouped-GEMM path (default 65, i.e. T <= 64 runs the
+    expert GEMVs); for tests and sweeps.  Returns the old value."""
+    old = int(lib().xb_set_moe_grouped_min_tokens(c_i32(min_tokens)))
+    _need(old >= 1, f"set_moe_grouped_min_tokens: {lib().xb_last_error().decode()}")
+    return old
+
+
+def moe_experts_describe(kind: str, T: int, k: int, H: int, I: int, E_local: int) -> str:
+    """host-only: the path the MoE expert entries take for a shape ("bf16 gemv", "w4 grouped bn=128 m_tiles<=40");
+    kind "bf16" or "w4"."""
+    buf = ctypes.create_string_buffer(96)
+    n = lib().xb_moe_experts_describe(c_i32({"bf16": 0, "w4": 2}[kind]), c_i32(T), c_i32(k), c_i32(H), c_i32(I), c_i32(E_local),
+                                      buf, c_i32(96))
+    _need(n > 0, "moe_experts_describe failed")
+    return buf.value.decode()
+
+
 def cutlass_fused_moe(input, token_selected_experts, token_final_scales, fc1_expert_weights, fc2_expert_weights, ep_size: int = 1,
                       ep_rank: int = 0, output=None, workspace=None):
-    """xllm::kernel::cuda::cutlass_fused_moe (cuda_ops_api.h:260-289) for unquantised bf16 experts and decode-sized token
-    counts: fc1 [E_local, 2I, H] ([up | gate]), fc2 [E_local, H, I]; experts of other EP ranks contribute zero."""
+    """xllm::kernel::cuda::cutlass_fused_moe (cuda_ops_api.h:260-289) for unquantised bf16 experts at any token count:
+    fc1 [E_local, 2I, H] ([up | gate]), fc2 [E_local, H, I]; experts of other EP ranks contribute zero.  T <= 64 runs one
+    expert GEMV per (token, expert) pair (decode); T >= 65 sorts the pairs by expert on the device and runs grouped wgmma
+    GEMMs (prefill).  No host synchronisation either way, so the call can be captured in a CUDA graph."""
     _cuda_bf16(input, "input"); _cuda_bf16(fc1_expert_weights, "fc1_expert_weights"); _cuda_bf16(fc2_expert_weights, "fc2_expert_weights")
     _need(token_selected_experts.dtype == torch.int32 and token_final_scales.dtype == torch.float32, "ids int32 / scales float32")
     _need(token_selected_experts.is_contiguous() and token_final_scales.is_contiguous() and fc1_expert_weights.is_contiguous() and
@@ -675,7 +695,8 @@ def cutlass_fused_moe(input, token_selected_experts, token_final_scales, fc1_exp
 def fused_moe_w4a16(input, token_selected_experts, token_final_scales, fc1_qweight, fc1_meta, fc2_qweight, fc2_meta, group_size,
                     ep_size: int = 1, ep_rank: int = 0, output=None, workspace=None):
     """W4A16 experts (additive; BASELINE configs[4]): fc1 [E_local, 2I/16, H/64, 32, 4] + meta [E_local, H/g, 2I] ([up | gate]
-    rows, quant.pack_w4 per expert), fc2 [E_local, H/16, I/64, 32, 4] + meta [E_local, I/g, H]."""
+    rows, quant.pack_w4 per expert), fc2 [E_local, H/16, I/64, 32, 4] + meta [E_local, I/g, H].  Same two paths as
+    cutlass_fused_moe: expert GEMVs for T <= 64, grouped wgmma GEMMs with the int4 dequantisation fused in above."""
     _cuda_bf16(input, "input")
     for t_, n in ((fc1_qweight, "fc1_qweight"), (fc1_meta, "fc1_meta"), (fc2_qweight, "fc2_qweight"), (fc2_meta, "fc2_meta")):
         _need(t_.is_cuda and t_.dtype == torch.int32 and t_.is_contiguous(), f"{n} must be contiguous int32 storage on device")
