@@ -199,6 +199,57 @@ int xb_paged_decode_bf16(const int64_t* plan8, const void* q, int64_t q_stride_n
                          float sm_scale, void* workspace_f32,
                          void* workspace_i32, xb_stream_t stream);
 
+/* ---- MLA (DeepSeek-V2/V3, Kimi-K2): latent cache writer + absorbed attention --
+ * additive (the reference runs MLA on MLU/NPU only; its CUDA cache layout is
+ * framework/kv_cache/kv_cache_shape.cpp:242-257,273-288): two paged caches,
+ * ckv_cache [pages, page_size, 512] = RMSNorm(c_kv) and kpe_cache
+ * [pages, page_size, 64] = RoPE(k_pe), element strides (page, token).
+ * Fixed dims kv_lora_rank = 512, qk_rope_head_dim = 64; others are rejected.
+ *
+ * xb_mla_cache_latent_bf16: fused_mla_kv with quant_mode "none"
+ * (kernels/param.h:1105-1180; non-fused form deepseek_v2_attention.cpp:223-240)
+ * in one launch.  latent [T, 576] (row stride) = kv_a_proj_with_mqa output
+ * [c_kv | k_pe]; gamma [512] = kv_a_layernorm; positions int64 [T];
+ * cos_sin_cache [max_pos, 64] = [cos | sin]; interleaved = 1 pairs (2i, 2i+1)
+ * (DeepSeek), 0 pairs (i, i+32) (NeoX); slot_ids int32 [T], slot < 0 skipped.
+ * Bit-identical to xb_rms_norm_bf16 + xb_rotary_embedding_bf16 + two
+ * xb_reshape_paged_cache_bf16 on the same inputs. */
+int xb_mla_cache_latent_bf16(const void* latent, int64_t latent_stride, const void* gamma, float eps,
+                             const int64_t* positions, const void* cos_sin_cache, int interleaved,
+                             const int32_t* slot_ids, void* ckv_cache, int64_t ckv_stride_page,
+                             int64_t ckv_stride_token, void* kpe_cache, int64_t kpe_stride_page,
+                             int64_t kpe_stride_token, int kv_lora_rank, int qk_rope_head_dim, int page_size,
+                             int num_tokens, xb_stream_t stream);
+/* xb_mla_plan: host-only arithmetic like xb_decode_plan.  Picks the KV-split
+ * count for batch requests of up to max_qo_len q tokens and num_heads heads
+ * (1..128) and returns the float workspace size in plan[1] bytes (0 without
+ * splits).  The split SIZE is derived on the device from the live kv_len, so a
+ * plan captured into a CUDA graph stays correct at later context lengths.
+ * xb_mla_plan_set_splits overrides the split count (1..128) and updates plan[1].
+ *
+ * xb_mla_paged_attention_bf16: absorbed MLA (layers/mlu/attention.cpp:65-155)
+ * over the paged caches: per q row, key = [c_kv | k_pe] of one kv head,
+ * value = c_kv; o = softmax(sm_scale [q_nope | q_pe] key^T) value.
+ * q_nope [T, H, 512] and q_pe [T, H, 64] take separate strides (the split form,
+ * or views of a packed q_input [T, H, 576]); o [T, H, 512] bf16.  Ragged q
+ * through qo_indptr [batch+1] (qo_len <= the plan's max_qo_len: q rows past
+ * it are not computed, and nothing is written outside o and the workspace); the paged
+ * triplet as in xb_paged_decode_bf16.  causal: q row i of a request sees
+ * kv <= kv_len - qo_len + i.  Serves decode (qo_len 1), speculative steps and
+ * chunked prefill; requests with kv_len 0 produce zero rows.  No allocation,
+ * no host synchronisation, capturable. */
+int xb_mla_plan(int64_t* plan8, int batch, int num_heads, int kv_lora_rank, int qk_rope_head_dim, int max_qo_len,
+                int page_size, int max_pages_per_request, int num_sms);
+int xb_mla_plan_set_splits(int64_t* plan8, int splits);
+int xb_mla_paged_attention_bf16(const int64_t* plan8, const void* q_nope, int64_t q_nope_stride_t,
+                                int64_t q_nope_stride_h, const void* q_pe, int64_t q_pe_stride_t, int64_t q_pe_stride_h,
+                                const void* ckv_cache, int64_t ckv_stride_page, int64_t ckv_stride_token,
+                                const void* kpe_cache, int64_t kpe_stride_page, int64_t kpe_stride_token,
+                                const int32_t* qo_indptr, const int32_t* kv_indptr, const int32_t* kv_indices,
+                                const int32_t* kv_last_page_len, int causal, void* o, int64_t o_stride_t,
+                                int64_t o_stride_h, float sm_scale, void* workspace, int64_t workspace_bytes,
+                                xb_stream_t stream);
+
 /* ---- weight-only / dense linears for small M (decode) ----------------------
  * y[M,N] = x[M,K] . W^T (+ bias).  HBM-bound streaming kernels for M <= 64.
  * (reference: ColumnParallelLinearImpl/RowParallelLinearImpl::forward,

@@ -29,11 +29,23 @@ def specs(head_dims=(128, 64)):
     return out
 
 
+def mla_specs():
+    """the fa2 batch_mla module BatchMLAPagedAttentionWrapper(backend="fa2") loads for DeepSeek-V2/V3 (ckv 512, kpe 64):
+    the comparator of tests/test_gpu_mla.py and tools/mla_sweep.py"""
+    import torch
+    from flashinfer.jit.attention.modules import gen_batch_mla_module
+    bf = torch.bfloat16
+    return [gen_batch_mla_module("fa2", bf, bf, bf, torch.int32, 512, 64, False)]
+
+
 def main():
     set_env()
     os.makedirs(FI_BASE, exist_ok=True)
-    dims = tuple(int(a) for a in sys.argv[1:]) or (128, 64)
-    for s in specs(dims):
+    if sys.argv[1:] == ["mla"]:
+        todo = mla_specs()
+    else:
+        todo = specs(tuple(int(a) for a in sys.argv[1:]) or (128, 64)) + (mla_specs() if not sys.argv[1:] else [])
+    for s in todo:
         print("building", s.name, flush=True)
         s.build(verbose=False)
         print("  ->", s.jit_library_path, os.path.getsize(s.jit_library_path) >> 20, "MiB", flush=True)

@@ -35,6 +35,31 @@ __device__ __forceinline__ float block_sum(float v, float* smem /*[33]*/) {
 // kVec: 8 bf16 per thread per step, row kept in registers (<= kMaxVec steps),
 // otherwise re-read from L2 (rows > 16K elements).
 // ---------------------------------------------------------------------------
+// ss + sum of squares of the 8 bf16 of x (fp32, in element order)
+__device__ __forceinline__ float sumsq_bf16x8(float ss, const uint4& x) {
+  const uint32_t* xp = &x.x;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    float a = bf16lo(xp[j]), b = bf16hi(xp[j]);
+    ss += a * a + b * b;
+  }
+  return ss;
+}
+// 8 normalised outputs: bf16(x*rstd) then bf16 product with w (norm.cu:75-77,130-133)
+__device__ __forceinline__ uint4 rms_apply_bf16x8(const uint4& x, const uint4& w, float rstd) {
+  const uint32_t* xp = &x.x;
+  const uint32_t* wp = &w.x;
+  uint4 o;
+  uint32_t* op = &o.x;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    float a = round_bf16(bf16lo(xp[j]) * rstd) * bf16lo(wp[j]);
+    float b = round_bf16(bf16hi(xp[j]) * rstd) * bf16hi(wp[j]);
+    op[j] = pack_bf16x2(a, b);
+  }
+  return o;
+}
+
 template <bool kFusedAdd, bool kFp8Out, bool kRoundBeforeFp8>
 __global__ void __launch_bounds__(1024)
 rms_norm_vec_kernel(void* __restrict__ out_, __nv_bfloat16* __restrict__ input,
@@ -76,12 +101,7 @@ rms_norm_vec_kernel(void* __restrict__ out_, __nv_bfloat16* __restrict__ input,
           xp[j] = pack_bf16x2(bf16lo(xp[j]) + bf16lo(rp[j]), bf16hi(xp[j]) + bf16hi(rp[j]));
         res_v[idx] = x;
       }
-      const uint32_t* xp = &x.x;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        float a = bf16lo(xp[j]), b = bf16hi(xp[j]);
-        ss += a * a + b * b;
-      }
+      ss = sumsq_bf16x8(ss, x);
       xr[i] = x;
     }
   }
@@ -97,12 +117,7 @@ rms_norm_vec_kernel(void* __restrict__ out_, __nv_bfloat16* __restrict__ input,
         xp[j] = pack_bf16x2(bf16lo(xp[j]) + bf16lo(rp[j]), bf16hi(xp[j]) + bf16hi(rp[j]));
       res_v[idx] = x;
     }
-    const uint32_t* xp = &x.x;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      float a = bf16lo(xp[j]), b = bf16hi(xp[j]);
-      ss += a * a + b * b;
-    }
+    ss = sumsq_bf16x8(ss, x);
   }
   const float var = block_sum(ss, red);
   const float rstd = rsqrtf(var / (float)hidden_size + eps);
@@ -115,15 +130,7 @@ rms_norm_vec_kernel(void* __restrict__ out_, __nv_bfloat16* __restrict__ input,
     const uint32_t* xp = &x.x;
     const uint32_t* wp = &w.x;
     if (!kFp8Out) {
-      uint4 o;
-      uint32_t* op = &o.x;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        // bf16(x*rstd) then bf16 product with w (norm.cu:75-77,130-133)
-        float a = round_bf16(bf16lo(xp[j]) * rstd) * bf16lo(wp[j]);
-        float b = round_bf16(bf16hi(xp[j]) * rstd) * bf16hi(wp[j]);
-        op[j] = pack_bf16x2(a, b);
-      }
+      const uint4 o = rms_apply_bf16x8(x, w, rstd);
       uint4* dst = kFusedAdd ? in_v : reinterpret_cast<uint4*>(
                                           reinterpret_cast<__nv_bfloat16*>(out_) + tok * (int64_t)hidden_size);
       dst[idx] = o;
@@ -289,11 +296,15 @@ __global__ void fp8_scale_finish_kernel(float* scale_out) {
 // K9 rotary embedding.  rope.cu:27-137: scalar_t arithmetic => every product
 // and the final add/sub are rounded to bf16.
 // ---------------------------------------------------------------------------
+// rotated pair (x, y) -> (out[xi], out[yi]); in place when in == out
+__device__ __forceinline__ void rope_pair(const __nv_bfloat16* in, __nv_bfloat16* out, int xi, int yi, float c, float s) {
+  const float x = __bfloat162float(in[xi]);
+  const float y = __bfloat162float(in[yi]);
+  out[xi] = __float2bfloat16_rn(round_bf16(x * c) - round_bf16(y * s));
+  out[yi] = __float2bfloat16_rn(round_bf16(y * c) + round_bf16(x * s));
+}
 __device__ __forceinline__ void rope_pair(__nv_bfloat16* arr, int xi, int yi, float c, float s) {
-  const float x = __bfloat162float(arr[xi]);
-  const float y = __bfloat162float(arr[yi]);
-  arr[xi] = __float2bfloat16_rn(round_bf16(x * c) - round_bf16(y * s));
-  arr[yi] = __float2bfloat16_rn(round_bf16(y * c) + round_bf16(x * s));
+  rope_pair(arr, arr, xi, yi, c, s);
 }
 
 template <bool kNeox>
@@ -606,6 +617,48 @@ act_and_mul_interleaved8_kernel(__nv_bfloat16* __restrict__ out, const __nv_bflo
   }
 }
 
+// ---------------------------------------------------------------------------
+// MLA latent cache writer (DeepSeek-V2/V3): the kv_a_proj_with_mqa row [c_kv 512 | k_pe 64] ->
+//   ckv_cache[slot] = RMSNorm(c_kv) (kv_a_layernorm), kpe_cache[slot] = RoPE(k_pe); slot < 0 skipped.
+// One launch for what rms_norm + rotary_embedding + two reshape_paged_cache do (fused_mla_kv with quant_mode "none",
+// kernels/param.h:1105-1180; non-fused form layers/mlu/deepseek_v2_attention.cpp:223-240).  64 threads per token: the
+// norm uses the thread mapping, accumulation order and rounding of rms_norm_vec_kernel at hidden size 512 (64 threads
+// of 8 elements) and RoPE is rope_pair, so both halves are bit-identical to the unfused kernels.
+// ---------------------------------------------------------------------------
+template <bool kNeox>
+__global__ void __launch_bounds__(64)
+mla_cache_latent_kernel(const __nv_bfloat16* __restrict__ latent, int64_t latent_stride,
+                        const __nv_bfloat16* __restrict__ gamma, float eps, const int64_t* __restrict__ positions,
+                        const __nv_bfloat16* __restrict__ cos_sin_cache, const int32_t* __restrict__ slot_ids,
+                        __nv_bfloat16* __restrict__ ckv_cache, int64_t ckv_stride_page, int64_t ckv_stride_token,
+                        __nv_bfloat16* __restrict__ kpe_cache, int64_t kpe_stride_page, int64_t kpe_stride_token,
+                        int page_size) {
+  constexpr int kDc = 512, kRot = 64;
+  __shared__ float red[33];
+  const int64_t tok = blockIdx.x;
+  const uint4 w = __ldg(reinterpret_cast<const uint4*>(gamma) + threadIdx.x);  // weights before the PDL wait
+  pdl_launch_dependents();
+  pdl_wait();
+  const int64_t slot = slot_ids[tok];
+  if (slot < 0) return;  // uniform over the CTA
+  const __nv_bfloat16* row = latent + tok * latent_stride;
+  const uint4 x = reinterpret_cast<const uint4*>(row)[threadIdx.x];
+  const float var = block_sum(sumsq_bf16x8(0.f, x), red);
+  const float rstd = rsqrtf(var / (float)kDc + eps);
+  const int64_t page = slot / page_size, off = slot % page_size;
+  reinterpret_cast<uint4*>(ckv_cache + page * ckv_stride_page + off * ckv_stride_token)[threadIdx.x] =
+      rms_apply_bf16x8(x, w, rstd);
+  if (threadIdx.x < kRot / 2) {
+    const int r = threadIdx.x;
+    const __nv_bfloat16* cs = cos_sin_cache + positions[tok] * kRot;
+    const float c = __bfloat162float(cs[r]), sn = __bfloat162float(cs[kRot / 2 + r]);
+    __nv_bfloat16* dst = kpe_cache + page * kpe_stride_page + off * kpe_stride_token;
+    if (kNeox) rope_pair(row + kDc, dst, r, kRot / 2 + r, c, sn);
+    else rope_pair(row + kDc, dst, 2 * r, 2 * r + 1, c, sn);
+  }
+  pdl_launch_dependents();
+}
+
 }  // namespace xb
 
 // ===========================================================================
@@ -813,5 +866,34 @@ extern "C" int xb_act_and_mul_interleaved8_bf16(void* out, const void* input, in
   if (act_mode == 0) XB_CUDA_OK(launch(act_and_mul_interleaved8_kernel<0>, grid, block, 0, s, true, o, in, d));
   else if (act_mode == 1) XB_CUDA_OK(launch(act_and_mul_interleaved8_kernel<1>, grid, block, 0, s, true, o, in, d));
   else XB_CUDA_OK(launch(act_and_mul_interleaved8_kernel<2>, grid, block, 0, s, true, o, in, d));
+  return 0;
+}
+
+extern "C" int xb_mla_cache_latent_bf16(const void* latent, int64_t latent_stride, const void* gamma, float eps,
+                                        const int64_t* positions, const void* cos_sin_cache, int interleaved,
+                                        const int32_t* slot_ids, void* ckv_cache, int64_t ckv_stride_page,
+                                        int64_t ckv_stride_token, void* kpe_cache, int64_t kpe_stride_page,
+                                        int64_t kpe_stride_token, int kv_lora_rank, int qk_rope_head_dim, int page_size,
+                                        int num_tokens, xb_stream_t stream) {
+  XB_CHECK(kv_lora_rank == 512 && qk_rope_head_dim == 64,
+           "mla_cache_latent: kv_lora_rank %d / qk_rope_head_dim %d unsupported (512 / 64)", kv_lora_rank,
+           qk_rope_head_dim);
+  XB_CHECK(num_tokens >= 0 && page_size >= 1, "mla_cache_latent: bad num_tokens %d or page_size %d", num_tokens,
+           page_size);
+  if (num_tokens == 0) return 0;
+  XB_CHECK(latent && gamma && positions && cos_sin_cache && slot_ids && ckv_cache && kpe_cache,
+           "mla_cache_latent: null pointer argument");
+  XB_CHECK(aligned16(latent) && aligned16(gamma) && aligned16(ckv_cache) && aligned16(kpe_cache) &&
+               latent_stride % 8 == 0 && ckv_stride_page % 8 == 0 && ckv_stride_token % 8 == 0,
+           "mla_cache_latent: latent, gamma and ckv_cache rows must be 16-byte aligned");
+  auto* lat = reinterpret_cast<const __nv_bfloat16*>(latent);
+  auto* g = reinterpret_cast<const __nv_bfloat16*>(gamma);
+  auto* cs = reinterpret_cast<const __nv_bfloat16*>(cos_sin_cache);
+  auto* ckv = reinterpret_cast<__nv_bfloat16*>(ckv_cache);
+  auto* kpe = reinterpret_cast<__nv_bfloat16*>(kpe_cache);
+  auto kern = interleaved ? mla_cache_latent_kernel<false> : mla_cache_latent_kernel<true>;
+  XB_CUDA_OK(launch(kern, dim3(num_tokens), dim3(64), 0, (cudaStream_t)stream, true, lat, latent_stride, g, eps,
+                    positions, cs, slot_ids, ckv, ckv_stride_page, ckv_stride_token, kpe, kpe_stride_page,
+                    kpe_stride_token, page_size));
   return 0;
 }

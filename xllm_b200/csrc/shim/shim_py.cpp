@@ -44,6 +44,13 @@ torch::Tensor cutlass_fused_moe(const torch::Tensor& input, const torch::Tensor&
                                 const std::optional<torch::Tensor>& output, bool enable_alltoall, bool use_deepseek_fp8_block_scale,
                                 bool use_w4_group_scaling, bool use_mxfp8_act_scaling, bool min_latency_mode, bool use_packed_weights,
                                 int32_t tune_max_num_tokens, ActivationType activation_type);
+void fused_mla_kv(const torch::Tensor& input_kv, const torch::Tensor& cos_sin_cache, const torch::Tensor& position_id,
+                  const torch::Tensor& gamma, torch::Tensor& k_cache, torch::Tensor& v_cache, const torch::Tensor& slot_mapping,
+                  const std::string& quant_mode, double eps, bool interleaved);
+void mla_paged_attention(const torch::Tensor& q_nope, const torch::Tensor& q_pe, const torch::Tensor& ckv_cache,
+                         const torch::Tensor& kpe_cache, const torch::Tensor& qo_indptr, const torch::Tensor& paged_kv_indptr,
+                         const torch::Tensor& paged_kv_indices, const torch::Tensor& paged_kv_last_page_len, int64_t max_qo_len,
+                         double sm_scale, bool causal, torch::Tensor& output);
 }  // namespace xllm::kernel::cuda
 
 namespace xk = xllm::kernel::cuda;
@@ -88,4 +95,15 @@ PYBIND11_MODULE(xllm_b200_shim_py, m) {
   }, pybind11::arg("input"), pybind11::arg("token_selected_experts"), pybind11::arg("token_final_scales"),
      pybind11::arg("fc1_expert_weights"), pybind11::arg("fc2_expert_weights"), pybind11::arg("ep_size") = 1,
      pybind11::arg("ep_rank") = 0);
+  m.def("fused_mla_kv", [](torch::Tensor input_kv, torch::Tensor cos_sin_cache, torch::Tensor position_id, torch::Tensor gamma,
+                           torch::Tensor k_cache, torch::Tensor v_cache, torch::Tensor slot_mapping, const std::string& quant_mode,
+                           double eps, bool interleaved) {
+    xk::fused_mla_kv(input_kv, cos_sin_cache, position_id, gamma, k_cache, v_cache, slot_mapping, quant_mode, eps, interleaved);
+  });
+  m.def("mla_paged_attention", [](torch::Tensor q_nope, torch::Tensor q_pe, torch::Tensor ckv_cache, torch::Tensor kpe_cache,
+                                  torch::Tensor qo_indptr, torch::Tensor kv_indptr, torch::Tensor kv_indices, torch::Tensor kv_last_page_len,
+                                  int64_t max_qo_len, double sm_scale, bool causal, torch::Tensor output) {
+    xk::mla_paged_attention(q_nope, q_pe, ckv_cache, kpe_cache, qo_indptr, kv_indptr, kv_indices, kv_last_page_len, max_qo_len,
+                            sm_scale, causal, output);
+  });
 }

@@ -12,6 +12,7 @@
 #include <c10/cuda/CUDAGuard.h>
 #include <torch/torch.h>
 
+#include <algorithm>
 #include <optional>
 #include <string>
 #include <tuple>
@@ -437,6 +438,83 @@ torch::Tensor cutlass_fused_moe(const torch::Tensor& input, const torch::Tensor&
      "cutlass_fused_moe");
   (void)ep_size;
   return out;
+}
+
+// ---- MLA (additive: the CUDA two-cache layout of kv_cache_shape.cpp:242-257,273-288) ----------------------------------------
+// fused_mla_kv (ops_api.h:112, FusedMlaKVParams param.h:1105-1180) for quant_mode "none" and a paged cache: input_kv
+// [T, 576] = [c_kv | k_pe], gamma [512], position_id int64 [T], the [cos | sin] table [max_pos, 64] the CUDA RoPE ops use,
+// k_cache = ckv_cache [blocks, block_size, (1,) 512], v_cache = kpe_cache [blocks, block_size, (1,) 64].
+void fused_mla_kv(const torch::Tensor& input_kv, const torch::Tensor& cos_sin_cache, const torch::Tensor& position_id,
+                  const torch::Tensor& gamma, torch::Tensor& k_cache, torch::Tensor& v_cache, const torch::Tensor& slot_mapping,
+                  const std::string& quant_mode, double eps, bool interleaved) {
+  TORCH_CHECK(quant_mode == "none", "fused_mla_kv: only quant_mode \"none\" is supported, got ", quant_mode);
+  need_bf16(input_kv, "input_kv");
+  need_bf16(cos_sin_cache, "cos_sin_cache");
+  need_bf16(gamma, "gamma");
+  need_bf16(k_cache, "k_cache");
+  need_bf16(v_cache, "v_cache");
+  need_dtype(position_id, torch::kInt64, "position_id");
+  need_dtype(slot_mapping, torch::kInt32, "slot_mapping");
+  const auto in = input_kv.reshape({-1, input_kv.size(-1)});
+  TORCH_CHECK(in.stride(1) == 1, "fused_mla_kv: input_kv rows must be contiguous");
+  const int64_t T = in.size(0);
+  TORCH_CHECK(position_id.numel() == T && slot_mapping.numel() == T, "fused_mla_kv: position_id / slot_mapping need one entry per token");
+  const auto ckv = k_cache.reshape({k_cache.size(0), k_cache.size(1), -1});
+  const auto kpe = v_cache.reshape({v_cache.size(0), v_cache.size(1), -1});
+  TORCH_CHECK(ckv.stride(2) == 1 && kpe.stride(2) == 1 && in.size(1) == ckv.size(2) + kpe.size(2) &&
+                  cos_sin_cache.size(-1) == kpe.size(2) && gamma.numel() == ckv.size(2),
+              "fused_mla_kv: shapes: input_kv [T, ", in.size(1), "], k_cache rows ", ckv.size(2), ", v_cache rows ", kpe.size(2));
+  XB_GUARD(input_kv);
+  ok(xb_mla_cache_latent_bf16(in.data_ptr(), in.stride(0), gamma.data_ptr(), (float)eps, position_id.data_ptr<int64_t>(),
+                              cos_sin_cache.data_ptr(), interleaved ? 1 : 0, slot_mapping.data_ptr<int32_t>(), ckv.data_ptr(),
+                              ckv.stride(0), ckv.stride(1), kpe.data_ptr(), kpe.stride(0), kpe.stride(1), (int)ckv.size(2),
+                              (int)kpe.size(2), (int)ckv.size(1), (int)T, stream()),
+     "fused_mla_kv");
+}
+
+// Absorbed MLA attention over the two paged caches: q_nope [T, H, 512], q_pe [T, H, 64] (any strides with unit last dim),
+// the ragged q / paged kv quadruple int32 on device, output [T, H, 512].  Plans (host-only) for max_qo_len and allocates
+// the split workspace when the plan asks for one; layers that capture graphs call the C ABI with a persistent plan.
+void mla_paged_attention(const torch::Tensor& q_nope, const torch::Tensor& q_pe, const torch::Tensor& ckv_cache,
+                         const torch::Tensor& kpe_cache, const torch::Tensor& qo_indptr, const torch::Tensor& paged_kv_indptr,
+                         const torch::Tensor& paged_kv_indices, const torch::Tensor& paged_kv_last_page_len, int64_t max_qo_len,
+                         double sm_scale, bool causal, torch::Tensor& output) {
+  need_bf16(q_nope, "q_nope");
+  need_bf16(q_pe, "q_pe");
+  need_bf16(ckv_cache, "ckv_cache");
+  need_bf16(kpe_cache, "kpe_cache");
+  need_bf16(output, "output");
+  need_dtype(qo_indptr, torch::kInt32, "qo_indptr");
+  need_dtype(paged_kv_indptr, torch::kInt32, "paged_kv_indptr");
+  need_dtype(paged_kv_indices, torch::kInt32, "paged_kv_indices");
+  need_dtype(paged_kv_last_page_len, torch::kInt32, "paged_kv_last_page_len");
+  TORCH_CHECK(q_nope.dim() == 3 && q_pe.dim() == 3 && output.dim() == 3 && q_nope.size(0) == q_pe.size(0) &&
+                  q_nope.size(1) == q_pe.size(1) && output.size(0) == q_nope.size(0) && output.size(1) == q_nope.size(1),
+              "mla_paged_attention: q_nope / q_pe / output must be [T, H, D] with equal T and H");
+  TORCH_CHECK(q_nope.stride(2) == 1 && q_pe.stride(2) == 1 && output.stride(2) == 1, "mla_paged_attention: last dims must be contiguous");
+  const auto ckv = ckv_cache.reshape({ckv_cache.size(0), ckv_cache.size(1), -1});
+  const auto kpe = kpe_cache.reshape({kpe_cache.size(0), kpe_cache.size(1), -1});
+  TORCH_CHECK(ckv.stride(2) == 1 && kpe.stride(2) == 1 && output.size(2) == ckv.size(2) && q_nope.size(2) == ckv.size(2) &&
+                  q_pe.size(2) == kpe.size(2),
+              "mla_paged_attention: q_nope / output width must equal the ckv_cache row, q_pe width the kpe_cache row");
+  const int64_t batch = paged_kv_indptr.numel() - 1;
+  TORCH_CHECK(batch >= 1 && qo_indptr.numel() == batch + 1 && paged_kv_last_page_len.numel() == batch,
+              "mla_paged_attention: qo_indptr [B+1], paged_kv_indptr [B+1], paged_kv_last_page_len [B]");
+  XB_GUARD(q_nope);
+  int64_t plan[8];
+  const int max_pages = (int)std::max<int64_t>(1, paged_kv_indices.numel());
+  ok(xb_mla_plan(plan, (int)batch, (int)q_nope.size(1), (int)ckv.size(2), (int)kpe.size(2), (int)max_qo_len, (int)ckv.size(1),
+                 max_pages, at::cuda::getCurrentDeviceProperties()->multiProcessorCount),
+     "mla_paged_attention");
+  torch::Tensor ws;
+  if (plan[1] > 0) ws = torch::empty({plan[1]}, torch::dtype(torch::kUInt8).device(q_nope.device()));
+  ok(xb_mla_paged_attention_bf16(plan, q_nope.data_ptr(), q_nope.stride(0), q_nope.stride(1), q_pe.data_ptr(), q_pe.stride(0),
+                                 q_pe.stride(1), ckv.data_ptr(), ckv.stride(0), ckv.stride(1), kpe.data_ptr(), kpe.stride(0),
+                                 kpe.stride(1), qo_indptr.data_ptr<int32_t>(), paged_kv_indptr.data_ptr<int32_t>(),
+                                 paged_kv_indices.data_ptr<int32_t>(), paged_kv_last_page_len.data_ptr<int32_t>(), causal ? 1 : 0,
+                                 output.data_ptr(), output.stride(0), output.stride(1), (float)sm_scale,
+                                 ws.defined() ? ws.data_ptr() : nullptr, plan[1], stream()),
+     "mla_paged_attention");
 }
 
 }  // namespace xllm::kernel::cuda

@@ -237,6 +237,75 @@ def batch_decode(plan: DecodePlan, query, k_cache, v_cache, paged_kv_indptr, pag
                                      _p(plan.int_ws), _stream()), "batch_decode")
 
 
+# ---- MLA (DeepSeek-V2/V3): latent cache writer + paged absorbed attention --------
+MLA_KV_LORA_RANK = 512
+MLA_ROPE_DIM = 64
+
+
+def mla_cache_latent(latent, gamma, eps: float, positions, cos_sin_cache, slot_ids, ckv_cache, kpe_cache,
+                     interleaved: bool = True) -> None:
+    """fused_mla_kv (kernels/param.h:1105-1180), quant_mode "none", CUDA two-cache layout: ckv_cache[slot] =
+    rms_norm(latent[:, :512], gamma), kpe_cache[slot] = rope(latent[:, 512:]); slot < 0 skipped.
+    latent [T, 576] (row stride allowed); caches [pages, page_size, 512] / [pages, page_size, 64] (or with a
+    singleton kv-head dim)."""
+    for t, n in ((latent, "latent"), (gamma, "gamma"), (cos_sin_cache, "cos_sin_cache"), (ckv_cache, "ckv_cache"),
+                 (kpe_cache, "kpe_cache")):
+        _cuda_bf16(t, n)
+    _need(positions.dtype == torch.int64 and slot_ids.dtype == torch.int32, "positions int64 / slot_ids int32")
+    _need(latent.dim() == 2 and latent.stride(1) == 1, "latent must be [T, 576] with unit column stride")
+    T = latent.size(0)
+    _need(positions.numel() == T and slot_ids.numel() == T, "positions / slot_ids need one entry per latent row")
+    ckv, kpe = ckv_cache.reshape(ckv_cache.size(0), ckv_cache.size(1), -1), kpe_cache.reshape(kpe_cache.size(0), kpe_cache.size(1), -1)
+    _need(ckv.stride(2) == 1 and kpe.stride(2) == 1, "cache rows must be contiguous")
+    _need(latent.size(1) == ckv.size(2) + kpe.size(2) and cos_sin_cache.size(-1) == kpe.size(2),
+          "latent must be [T, kv_lora_rank + rope_dim], cos_sin_cache [max_pos, rope_dim]")
+    check(lib().xb_mla_cache_latent_bf16(_p(latent), c_i64(latent.stride(0)), _p(gamma), c_f32(eps), _p(positions),
+                                         _p(cos_sin_cache), c_i32(1 if interleaved else 0), _p(slot_ids), _p(ckv),
+                                         c_i64(ckv.stride(0)), c_i64(ckv.stride(1)), _p(kpe), c_i64(kpe.stride(0)),
+                                         c_i64(kpe.stride(1)), c_i32(ckv.size(2)), c_i32(kpe.size(2)), c_i32(ckv.size(1)), c_i32(T), _stream()),
+          "mla_cache_latent")
+
+
+class MlaPlan:
+    """Host-only plan of mla_paged_attention (split count + workspace); valid for any later context length."""
+
+    def __init__(self, batch, num_heads, max_qo_len, page_size, max_pages_per_request, device,
+                 num_sms: Optional[int] = None, splits: Optional[int] = None):
+        if num_sms is None:
+            num_sms = torch.cuda.get_device_properties(device).multi_processor_count
+        self.arr = (ctypes.c_int64 * 8)()
+        check(lib().xb_mla_plan(self.arr, c_i32(batch), c_i32(num_heads), c_i32(MLA_KV_LORA_RANK), c_i32(MLA_ROPE_DIM),
+                                c_i32(max_qo_len), c_i32(page_size), c_i32(max_pages_per_request), c_i32(num_sms)),
+              "mla_plan")
+        if splits is not None:
+            check(lib().xb_mla_plan_set_splits(self.arr, c_i32(splits)), "mla_plan_set_splits")
+        self.splits, self.workspace_bytes = int(self.arr[0]), int(self.arr[1])
+        self.workspace = torch.empty(max(self.workspace_bytes, 16), dtype=torch.uint8, device=device)
+
+
+def mla_paged_attention(plan: MlaPlan, q_nope, q_pe, ckv_cache, kpe_cache, qo_indptr, paged_kv_indptr, paged_kv_indices,
+                        paged_kv_last_page_len, sm_scale: float, output, causal: bool = True) -> None:
+    """Absorbed MLA over the paged latent caches: q_nope [T, H, 512], q_pe [T, H, 64] (separate strides: split tensors
+    or views of a packed [T, H, 576] q_input), output [T, H, 512]."""
+    for t, n in ((q_nope, "q_nope"), (q_pe, "q_pe"), (ckv_cache, "ckv_cache"), (kpe_cache, "kpe_cache"), (output, "output")):
+        _cuda_bf16(t, n)
+    for t, n in ((qo_indptr, "qo_indptr"), (paged_kv_indptr, "paged_kv_indptr"), (paged_kv_indices, "paged_kv_indices"),
+                 (paged_kv_last_page_len, "paged_kv_last_page_len")):
+        _need(t.dtype == torch.int32 and t.is_cuda, f"{n} must be int32 on device")
+    _need(q_nope.dim() == 3 and q_pe.dim() == 3 and output.dim() == 3, "q_nope / q_pe / output must be [T, H, D]")
+    _need(q_nope.size(2) == MLA_KV_LORA_RANK and q_pe.size(2) == MLA_ROPE_DIM and output.size(2) == MLA_KV_LORA_RANK,
+          "MLA dims are kv_lora_rank 512 / qk_rope_head_dim 64")
+    _need(q_nope.stride(2) == 1 and q_pe.stride(2) == 1 and output.stride(2) == 1, "last dims must be contiguous")
+    ckv, kpe = ckv_cache.reshape(ckv_cache.size(0), ckv_cache.size(1), -1), kpe_cache.reshape(kpe_cache.size(0), kpe_cache.size(1), -1)
+    _need(ckv.stride(2) == 1 and kpe.stride(2) == 1, "cache rows must be contiguous")
+    check(lib().xb_mla_paged_attention_bf16(
+        plan.arr, _p(q_nope), c_i64(q_nope.stride(0)), c_i64(q_nope.stride(1)), _p(q_pe), c_i64(q_pe.stride(0)),
+        c_i64(q_pe.stride(1)), _p(ckv), c_i64(ckv.stride(0)), c_i64(ckv.stride(1)), _p(kpe), c_i64(kpe.stride(0)),
+        c_i64(kpe.stride(1)), _p(qo_indptr), _p(paged_kv_indptr), _p(paged_kv_indices), _p(paged_kv_last_page_len),
+        c_i32(1 if causal else 0), _p(output), c_i64(output.stride(0)), c_i64(output.stride(1)), c_f32(sm_scale),
+        _p(plan.workspace), c_i64(plan.workspace.numel()), _stream()), "mla_paged_attention")
+
+
 # ---- linears ------------------------------------------------------------------
 def matmul_small_m(a, b, bias=None, out=None):
     """xllm::kernel::cuda::matmul (cuda_ops_api.h:167-169, matmul.cpp:20-24) for M <= 64: a [M,K], b [N,K]."""
