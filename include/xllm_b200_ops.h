@@ -249,6 +249,55 @@ int xb_mla_paged_attention_bf16(const int64_t* plan8, const void* q_nope, int64_
                                 const int32_t* kv_last_page_len, int causal, void* o, int64_t o_stride_t,
                                 int64_t o_stride_h, float sm_scale, void* workspace, int64_t workspace_bytes,
                                 xb_stream_t stream);
+/* Expanded MLA prefill (DeepSeek-V3 attention as transformers' DeepseekV3Attention
+ * computes it): the latent rows are up-projected through kv_b_proj into per-head
+ * k_nope / v, then ordinary causal attention runs with 192-wide QK
+ * ([q_nope | q_pe] . [k_nope | k_pe], k_pe shared by all heads) and 128-wide V.
+ * qk_nope_head_dim = v_head_dim = 128 (kv_b_proj [H * 256, 512]), kv_lora_rank 512,
+ * qk_rope_head_dim 64.
+ *
+ * xb_mla_expanded_plan: host-only.  qo_lens_host / kv_lens_host [batch] are the
+ * step's q lengths and the total kv lengths (history + the step's tokens,
+ * qo_len <= kv_len).  plan8: [0] use_expanded, [1] workspace bytes, [2] batch,
+ * [3] num_heads, [4] max_qo_len, [5] total_kv, [6] max_kv_len, [7] total_q | tag.
+ *   use_expanded = max_qo_len > 1 and  F_abs > 0.5 * (F_up + F_exp), with per
+ *   head F_abs = 2 (576 + 512) P, F_exp = 2 (192 + 128) P, F_up = 2 * 512 * 256 *
+ *   total_kv, P = the causal (q, kv) pairs: one FLOP of the expanded path is
+ *   taken to cost as much as 0.5 FLOP of the absorbed kernel.  The constant
+ *   gives the least total time over the selector grid of tools/mla_sweep.py
+ *   (README).  Decode steps and short chunks over long histories come out
+ *   absorbed (xb_mla_paged_attention_bf16); long prompts expanded.  The form and
+ *   the sizes do not depend on the SM count, so the plan takes none.
+ *   The selector looks at FLOPs only: the workspace grows as total_kv * H * 512
+ *   bytes (8.9 GB for 4096 new tokens over 128 K of history at H = 128); a
+ *   caller short of memory compares plan[1] with what it can spare and runs
+ *   the absorbed form instead.
+ *   Workspace layout, every part 256-byte aligned:
+ *     kv_up [total_kv, H, 256] bf16 (per head k_nope | v) at byte 0,
+ *     ckv   [total_kv, 512] bf16 at align256(total_kv * H * 512),
+ *     kpe   [total_kv, 64] bf16 after it (align256(total_kv * 1024) further),
+ *     kv_cu int32 [batch + 1] after it (align256(total_kv * 128) further).
+ *
+ * xb_mla_prefill_expanded_bf16: three launches, no allocation, no host
+ * synchronisation.  q [T, H, 192] = [q_nope | roped q_pe] (row / head strides);
+ * the caches and the paged triplet as in xb_mla_paged_attention_bf16, holding
+ * the history and the step's tokens; qo_indptr [batch + 1]; kv_b_proj
+ * [H * 256, 512] (the checkpoint's kv_b_proj.weight); o [T, H, 128] = o_proj's
+ * input.  Causal: q row i of a request sees kv <= kv_len - qo_len + i.
+ *   1. gather: each request's c_kv / k_pe rows into the workspace's ckv / kpe,
+ *      row offsets from the device's lengths; rows past the plan's total_kv are
+ *      not written (the workspace is never written outside plan[1] bytes);
+ *   2. xb_gemm_bf16: kv_up = ckv . kv_b_proj^T;
+ *   3. attention on the 192 / 128 wgmma prefill kernel. */
+int xb_mla_expanded_plan(int64_t* plan8, int batch, int num_heads, const int32_t* qo_lens_host,
+                         const int32_t* kv_lens_host);
+int xb_mla_prefill_expanded_bf16(const int64_t* plan8, const void* q, int64_t q_stride_t, int64_t q_stride_h,
+                                 const void* ckv_cache, int64_t ckv_stride_page, int64_t ckv_stride_token,
+                                 const void* kpe_cache, int64_t kpe_stride_page, int64_t kpe_stride_token, int page_size,
+                                 const int32_t* kv_indptr, const int32_t* kv_indices, const int32_t* kv_last_page_len,
+                                 const int32_t* qo_indptr, const void* kv_b_proj, void* o, int64_t o_stride_t,
+                                 int64_t o_stride_h, float sm_scale, void* workspace, int64_t workspace_bytes,
+                                 xb_stream_t stream);
 
 /* ---- weight-only / dense linears for small M (decode) ----------------------
  * y[M,N] = x[M,K] . W^T (+ bias).  HBM-bound streaming kernels for M <= 64.

@@ -38,13 +38,24 @@ def mla_specs():
     return [gen_batch_mla_module("fa2", bf, bf, bf, torch.int32, 512, 64, False)]
 
 
+def mla_prefill_specs():
+    """the fa2 ragged prefill module BatchPrefillWithRaggedKVCacheWrapper(backend="fa2") loads for DeepSeek-V3's expanded
+    MLA prefill (head_dim_qk 192, head_dim_vo 128): the comparator of tests/test_gpu_mla_prefill.py and tools/mla_sweep.py"""
+    import torch
+    from flashinfer.jit.attention.modules import gen_batch_prefill_module
+    bf = torch.bfloat16
+    return [gen_batch_prefill_module("fa2", bf, bf, bf, torch.int32, 192, 128, 0, False, False, False)]
+
+
 def main():
     set_env()
     os.makedirs(FI_BASE, exist_ok=True)
     if sys.argv[1:] == ["mla"]:
         todo = mla_specs()
+    elif sys.argv[1:] == ["mla_prefill"]:
+        todo = mla_prefill_specs()
     else:
-        todo = specs(tuple(int(a) for a in sys.argv[1:]) or (128, 64)) + (mla_specs() if not sys.argv[1:] else [])
+        todo = specs(tuple(int(a) for a in sys.argv[1:]) or (128, 64)) + (mla_specs() + mla_prefill_specs() if not sys.argv[1:] else [])
     for s in todo:
         print("building", s.name, flush=True)
         s.build(verbose=False)

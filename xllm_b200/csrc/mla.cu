@@ -14,7 +14,11 @@
 // Split-KV: the plan fixes the split COUNT; the split size is derived here from the live kv_len, so a plan captured into
 // a CUDA graph stays valid at later context lengths.  Partials (normalised fp32 O + base-2 LSE) meet in a separate merge
 // kernel that sums them in split order (run-to-run bit-identical), as prefill_attention.cu does.
-#include "common.cuh"
+//
+// Expanded prefill (xb_mla_prefill_expanded_bf16): the latent rows are gathered into a contiguous workspace, up-projected
+// through kv_b_proj into per-head [k_nope | v] by the wgmma GEMM, and attended by the 192 / 128 instantiation of the
+// prefill attention kernel: 2 (192 + 128) FLOP per (q, kv, head) instead of the absorbed form's 2 (576 + 512).
+#include "tc_common.cuh"
 
 namespace xb {
 namespace {
@@ -326,6 +330,95 @@ int64_t mla_workspace_bytes(int64_t splits, int64_t part_rows, int num_heads) {
   return splits > 1 ? splits * part_rows * num_heads * (kMlaDc + 1) * (int64_t)sizeof(float) : 0;
 }
 
+// ---- expanded prefill ------------------------------------------------------------------------------------------
+constexpr int kMlaUpW = 256;                 // kv_b_proj rows per head: k_nope 128 | v 128
+constexpr int kMlaGatherTokens = 32;
+constexpr int kMlaGatherThreads = 256;
+constexpr int64_t kMlaExpTag = 0x4D4C45;     // "MLE": plan8[7] >> 40
+// Selector: expanded when  absorbed FLOP > kMlaExpandedCost * (up-projection FLOP + expanded attention FLOP), i.e. one
+// FLOP of the expanded path costs as much time as kMlaExpandedCost FLOP of the absorbed kernel.  Criterion: the least total
+// time over the selector grid of tools/mla_sweep.py (H100 80GB HBM3, 700 W; README).  Every constant from 0.13 to 0.80
+// reaches it (63.84 ms; the qo = 128 / history 0 points, FLOP ratio 0.463, split that range and move the total by 1.6 us),
+// and 0.5 lies amid the break-even ratios measured for chunks of 512+ tokens (0.37-0.68).  Worst point: a 128-token
+// chunk over 32 K history at H = 16 runs expanded, 1.40x slower than absorbed.
+constexpr double kMlaExpandedCost = 0.5;
+
+struct MlaGatherParams {
+  const __nv_bfloat16* ckv;
+  int64_t ckv_stride_page, ckv_stride_token;
+  const __nv_bfloat16* kpe;
+  int64_t kpe_stride_page, kpe_stride_token;
+  const int32_t* kv_indptr;
+  const int32_t* kv_indices;
+  const int32_t* kv_last_page_len;
+  int page_size;
+  int64_t total_kv;       // the plan's row capacity of ckv_out / kpe_out
+  __nv_bfloat16* ckv_out; // [total_kv, 512]
+  __nv_bfloat16* kpe_out; // [total_kv, 64]
+  int32_t* kv_cu;         // [batch + 1] ragged offsets of the gathered rows
+};
+
+__device__ __forceinline__ int64_t mla_kv_len(const MlaGatherParams& g, int b) {
+  const int n_pages = g.kv_indptr[b + 1] - g.kv_indptr[b];
+  return n_pages > 0 ? (int64_t)(n_pages - 1) * g.page_size + g.kv_last_page_len[b] : 0;
+}
+
+// One CTA per (32 kv tokens, request).  The request's first row is the sum of the live kv lengths before it; rows at or
+// past the plan's total_kv are not written, and kv_cu is clamped to total_kv, so lengths beyond the plan stay inside the
+// workspace.
+__global__ void __launch_bounds__(kMlaGatherThreads)
+mla_gather_latent_kernel(const MlaGatherParams g) {
+  __shared__ int64_t red[kMlaGatherThreads / 32];
+  const int b = blockIdx.y;
+  pdl_launch_dependents();
+  pdl_wait();
+  int64_t part = 0;
+  for (int i = threadIdx.x; i < b; i += kMlaGatherThreads) part += mla_kv_len(g, i);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = part;
+  __syncthreads();
+  int64_t off = 0;
+#pragma unroll
+  for (int w = 0; w < kMlaGatherThreads / 32; ++w) off += red[w];
+  const int64_t kv_len = mla_kv_len(g, b);
+  if (blockIdx.x == 0 && threadIdx.x == 0) {
+    g.kv_cu[b + 1] = (int32_t)min(off + kv_len, g.total_kv);
+    if (b == 0) g.kv_cu[0] = 0;
+  }
+  const int p0 = g.kv_indptr[b];
+  constexpr int kChunks = kMlaD / 8;  // 16-byte pieces of [c_kv | k_pe]
+  for (int c = threadIdx.x; c < kMlaGatherTokens * kChunks; c += kMlaGatherThreads) {
+    const int64_t t = (int64_t)blockIdx.x * kMlaGatherTokens + c / kChunks;
+    const int k = c % kChunks;
+    const int64_t row = off + t;
+    if (t >= kv_len || row >= g.total_kv) continue;
+    const int64_t pg = g.kv_indices[p0 + t / g.page_size], in_pg = t % g.page_size;
+    if (k < kMlaDc / 8)
+      *reinterpret_cast<uint4*>(g.ckv_out + row * kMlaDc + k * 8) =
+          *reinterpret_cast<const uint4*>(g.ckv + pg * g.ckv_stride_page + in_pg * g.ckv_stride_token + k * 8);
+    else
+      *reinterpret_cast<uint4*>(g.kpe_out + row * kMlaDr + (k - kMlaDc / 8) * 8) =
+          *reinterpret_cast<const uint4*>(g.kpe + pg * g.kpe_stride_page + in_pg * g.kpe_stride_token + (k - kMlaDc / 8) * 8);
+  }
+}
+
+int64_t align256(int64_t x) { return (x + 255) & ~int64_t(255); }
+
+// workspace layout (bytes): kv_up [total_kv, H, 256] bf16 at 0 | ckv [total_kv, 512] bf16 | kpe [total_kv, 64] bf16 |
+// kv_cu int32 [batch + 1]; each part starts on a 256-byte boundary
+struct MlaExpLayout {
+  int64_t ckv, kpe, kv_cu, bytes;
+};
+MlaExpLayout mla_exp_layout(int64_t total_kv, int num_heads, int batch) {
+  MlaExpLayout l;
+  l.ckv = align256(total_kv * num_heads * kMlaUpW * 2);
+  l.kpe = l.ckv + align256(total_kv * kMlaDc * 2);
+  l.kv_cu = l.kpe + align256(total_kv * kMlaDr * 2);
+  l.bytes = l.kv_cu + align256((int64_t)(batch + 1) * 4);
+  return l;
+}
+
 }  // namespace
 }  // namespace xb
 
@@ -435,4 +528,98 @@ extern "C" int xb_mla_paged_attention_bf16(const int64_t* plan8, const void* q_n
   p.part_lse = p.part_o ? p.part_o + (int64_t)p.splits * p.part_rows * p.num_heads * kMlaDc : nullptr;
   cudaStream_t s = (cudaStream_t)stream;
   return rg == 1 ? launch_mla<1>(p, m_tiles, s) : launch_mla<4>(p, m_tiles, s);
+}
+
+// plan8: [0] use_expanded  [1] workspace bytes  [2] batch  [3] num_heads  [4] max_qo_len  [5] total_kv  [6] max_kv_len
+//        [7] total_q | tag << 40
+extern "C" int xb_mla_expanded_plan(int64_t* plan8, int batch, int num_heads, const int32_t* qo_lens_host,
+                                    const int32_t* kv_lens_host) {
+  XB_CHECK(plan8 != nullptr, "mla_expanded_plan: plan8 is null");
+  XB_CHECK(num_heads >= 1 && num_heads <= 128, "mla_expanded_plan: num_heads %d unsupported (1..128)", num_heads);
+  XB_CHECK(batch >= 1 && batch <= 65535, "mla_expanded_plan: batch %d out of range (1..65535)", batch);
+  XB_CHECK(qo_lens_host != nullptr && kv_lens_host != nullptr, "mla_expanded_plan: null qo_lens / kv_lens");
+  int64_t total_q = 0, total_kv = 0, pairs = 0;
+  int max_qo = 0, max_kv = 0;
+  for (int b = 0; b < batch; ++b) {
+    const int64_t qo = qo_lens_host[b], kv = kv_lens_host[b];
+    XB_CHECK(qo >= 0 && kv >= qo, "mla_expanded_plan: request %d has qo_len %lld > kv_len %lld (or a negative length)", b,
+             (long long)qo, (long long)kv);
+    total_q += qo;
+    total_kv += kv;
+    pairs += qo * (kv - qo) + qo * (qo + 1) / 2;  // causal (q, kv) pairs
+    max_qo = qo > max_qo ? (int)qo : max_qo;
+    max_kv = kv > max_kv ? (int)kv : max_kv;
+  }
+  XB_CHECK(total_q <= INT32_MAX && total_kv <= INT32_MAX, "mla_expanded_plan: %lld q / %lld kv tokens exceed int32",
+           (long long)total_q, (long long)total_kv);
+  // FLOP per head: absorbed 2 (576 + 512) per pair; expanded 2 (192 + 128) per pair + 2 * 512 * 256 per kv token
+  const double absorbed = 2.0 * (kMlaD + kMlaDc) * (double)pairs;
+  const double expanded = 2.0 * (192 + 128) * (double)pairs + 2.0 * kMlaDc * kMlaUpW * (double)total_kv;
+  plan8[0] = max_qo > 1 && absorbed > kMlaExpandedCost * expanded ? 1 : 0;
+  plan8[1] = mla_exp_layout(total_kv, num_heads, batch).bytes;
+  plan8[2] = batch;
+  plan8[3] = num_heads;
+  plan8[4] = max_qo;
+  plan8[5] = total_kv;
+  plan8[6] = max_kv;
+  plan8[7] = total_q | (kMlaExpTag << 40);
+  return 0;
+}
+
+extern "C" int xb_mla_prefill_expanded_bf16(const int64_t* plan8, const void* q, int64_t q_stride_t, int64_t q_stride_h,
+                                            const void* ckv_cache, int64_t ckv_stride_page, int64_t ckv_stride_token,
+                                            const void* kpe_cache, int64_t kpe_stride_page, int64_t kpe_stride_token,
+                                            int page_size, const int32_t* kv_indptr, const int32_t* kv_indices,
+                                            const int32_t* kv_last_page_len, const int32_t* qo_indptr,
+                                            const void* kv_b_proj, void* o, int64_t o_stride_t, int64_t o_stride_h,
+                                            float sm_scale, void* workspace, int64_t workspace_bytes,
+                                            xb_stream_t stream) {
+  XB_CHECK(plan8 != nullptr && (plan8[7] >> 40) == kMlaExpTag,
+           "mla_prefill_expanded: plan is not an expanded MLA plan (xb_mla_expanded_plan)");
+  const int batch = (int)plan8[2], num_heads = (int)plan8[3], max_qo = (int)plan8[4], max_kv = (int)plan8[6];
+  const int64_t total_kv = plan8[5], total_q = plan8[7] & ((int64_t(1) << 40) - 1);
+  XB_CHECK(batch >= 1 && num_heads >= 1 && num_heads <= 128 && total_kv >= 0 && max_kv >= 0 &&
+               plan8[1] == mla_exp_layout(total_kv, num_heads, batch).bytes,
+           "mla_prefill_expanded: corrupt plan");
+  XB_CHECK(q && ckv_cache && kpe_cache && kv_b_proj && o, "mla_prefill_expanded: null q / cache / kv_b_proj / o pointer");
+  XB_CHECK(qo_indptr && kv_indptr && kv_indices && kv_last_page_len,
+           "mla_prefill_expanded: null qo_indptr / paged kv pointer");
+  XB_CHECK(page_size >= 1, "mla_prefill_expanded: page_size %d", page_size);
+  XB_CHECK(workspace != nullptr && workspace_bytes >= plan8[1],
+           "mla_prefill_expanded: workspace of %lld bytes is smaller than the plan's %lld", (long long)workspace_bytes,
+           (long long)plan8[1]);
+  const auto a16 = [](const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; };
+  XB_CHECK(a16(q) && a16(ckv_cache) && a16(kpe_cache) && a16(kv_b_proj) && a16(workspace) &&
+               (reinterpret_cast<uintptr_t>(o) & 3) == 0 && q_stride_t % 8 == 0 && q_stride_h % 8 == 0 &&
+               ckv_stride_page % 8 == 0 && ckv_stride_token % 8 == 0 && kpe_stride_page % 8 == 0 &&
+               kpe_stride_token % 8 == 0 && o_stride_t % 2 == 0 && o_stride_h % 2 == 0,
+           "mla_prefill_expanded: q / cache / kv_b_proj / workspace rows must be 16-byte aligned, o rows 4-byte aligned");
+  if (total_q == 0) return 0;
+  const MlaExpLayout l = mla_exp_layout(total_kv, num_heads, batch);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  auto* kv_up = reinterpret_cast<__nv_bfloat16*>(ws);
+  MlaGatherParams g{};
+  g.ckv = reinterpret_cast<const __nv_bfloat16*>(ckv_cache);
+  g.ckv_stride_page = ckv_stride_page;
+  g.ckv_stride_token = ckv_stride_token;
+  g.kpe = reinterpret_cast<const __nv_bfloat16*>(kpe_cache);
+  g.kpe_stride_page = kpe_stride_page;
+  g.kpe_stride_token = kpe_stride_token;
+  g.kv_indptr = kv_indptr;
+  g.kv_indices = kv_indices;
+  g.kv_last_page_len = kv_last_page_len;
+  g.page_size = page_size;
+  g.total_kv = total_kv;
+  g.ckv_out = reinterpret_cast<__nv_bfloat16*>(ws + l.ckv);
+  g.kpe_out = reinterpret_cast<__nv_bfloat16*>(ws + l.kpe);
+  g.kv_cu = reinterpret_cast<int32_t*>(ws + l.kv_cu);
+  cudaStream_t s = (cudaStream_t)stream;
+  const unsigned chunks = (unsigned)((max_kv + kMlaGatherTokens - 1) / kMlaGatherTokens);
+  XB_CUDA_OK(launch(mla_gather_latent_kernel, dim3(chunks > 0 ? chunks : 1, batch), dim3(kMlaGatherThreads), 0, s, true, g));
+  // kv_up [total_kv, H * 256] = ckv [total_kv, 512] . kv_b_proj [H * 256, 512]^T
+  if (xb_gemm_bf16(kv_up, (int64_t)num_heads * kMlaUpW, g.ckv_out, kMlaDc, kv_b_proj, nullptr, (int)total_kv,
+                   num_heads * kMlaUpW, kMlaDc, stream))
+    return 1;
+  return mla_expanded_attention(q, q_stride_t, q_stride_h, total_q, kv_up, g.kpe_out, total_kv, qo_indptr, g.kv_cu, o,
+                                o_stride_t, o_stride_h, batch, max_qo, num_heads, sm_scale, s);
 }

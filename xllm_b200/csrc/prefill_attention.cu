@@ -14,6 +14,10 @@
 //               (denominator summed from the ROUNDED P like the reference ladder) and kept in registers as the A operand
 //               of O += P V (V straight from its [kv, d] TMA tile as an MN-major operand - no transpose pass), final
 //               O / l -> bf16 -> global.
+// kDQK != kDV (192 / 128: expanded MLA prefill, group 1, ragged, kv_splits 1): Q [T, H, 192] is three 64-column sub-tiles;
+// a K tile is two 64-column sub-tiles of k_nope from tmap_k at column kvh * kv_head_stride plus one sub-tile of k_pe from
+// tmap_kr at column kvh * kr_head_stride (0: one k_pe row shared by all heads); a V tile is two sub-tiles from tmap_v at
+// column kvh * kv_head_stride + v_col_off.  So k_nope and v are read as strided views of the up-projection [N, H, 256].
 #include <type_traits>
 
 #include "tc_common.cuh"
@@ -42,29 +46,41 @@ struct PrefillParams {
   int64_t total_q;
 };
 
+// kDQK != kDV only: column offsets (elements) of a head's K / V parts, see the header comment
+struct KvColumns {
+  int kv_head_stride, v_col_off, kr_head_stride;
+};
+
 constexpr int kKT = 128;   // kv tile
 constexpr int kPrefillThreads = 384;
 
-template <int kD>
+template <int kDQK, int kDV>
 struct PrefillCfg {
-  static constexpr int kHalves = kD / 64;
+  static constexpr int kHalves = kDQK / 64;                        // sub-tiles of a Q or K tile
+  static constexpr int kVHalves = kDV / 64;
   static constexpr int kSub = 128 * 128;                           // one [128 rows x 64 elems] swizzled sub-tile
   static constexpr int kQBytes = kHalves * kSub;
-  static constexpr int kKVBytes = kHalves * kSub;                  // K tile or V tile
-  static constexpr int kSmemBytes = kQBytes + 4 * kKVBytes + 1024 + 256;
+  static constexpr int kKBytes = kHalves * kSub;
+  static constexpr int kVBytes = kVHalves * kSub;
+  static constexpr int kSmemBytes = kQBytes + 2 * kKBytes + 2 * kVBytes + 1024 + 256;
 };
 
-template <int kD>
+// tmap_kr (the shared k_pe rows) and kc are read only when kDQK != kDV.  They follow p, and PrefillParams keeps its
+// layout, so the kDQK == kDV instantiations compile to the code they had before the 192 / 128 variant existed.
+template <int kDQK, int kDV>
 __global__ void __launch_bounds__(kPrefillThreads, 1)
 prefill_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_constant__ CUtensorMap tmap_k,
-                         const __grid_constant__ CUtensorMap tmap_v, const PrefillParams p) {
-  using Cfg = PrefillCfg<kD>;
+                         const __grid_constant__ CUtensorMap tmap_v, const PrefillParams p,
+                         const __grid_constant__ CUtensorMap tmap_kr, const KvColumns kc) {
+  static_assert((kDQK == 64 && kDV == 64) || (kDQK == 128 && kDV == 128) || (kDQK == 192 && kDV == 128),
+                "prefill attention: QK / V widths 64 / 64, 128 / 128 or 192 / 128");
+  using Cfg = PrefillCfg<kDQK, kDV>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* q_s = smem;
-  uint8_t* k_s = q_s + Cfg::kQBytes;                // [2][kKVBytes]
-  uint8_t* v_s = k_s + 2 * Cfg::kKVBytes;           // [2][kKVBytes]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(v_s + 2 * Cfg::kKVBytes);
+  uint8_t* k_s = q_s + Cfg::kQBytes;                // [2][kKBytes]
+  uint8_t* v_s = k_s + 2 * Cfg::kKBytes;            // [2][kVBytes]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(v_s + 2 * Cfg::kVBytes);
   uint64_t* q_full = bars;            // 1
   uint64_t* k_full = bars + 1;        // 2
   uint64_t* k_empty = bars + 3;       // 2
@@ -89,6 +105,7 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gri
     tma_prefetch_desc(&tmap_q);
     tma_prefetch_desc(&tmap_k);
     tma_prefetch_desc(&tmap_v);
+    if constexpr (kDQK != kDV) tma_prefetch_desc(&tmap_kr);
   }
   __syncthreads();
   pdl_launch_dependents();
@@ -119,10 +136,14 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gri
   const int n_tiles = max(0, min(per_split, n_tiles_all - j0));
   const int rows_used = p.tokens_per_tile * p.group;
 
+  // 192 / 128: the consumers' 128 fp32 accumulators and the wider Q / K addressing do not fit the 168 registers that
+  // __launch_bounds__(384, 1) leaves (65536 / 384, rounded down to 8), so warpgroup 0, which only issues TMA, hands
+  // registers to the two consumer warpgroups: 128 x 40 + 256 x 232 = 384 x 168.
   if (warp == 0) {
+    if constexpr (kDQK != kDV) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");
     // ============================== TMA producer ==============================
     if (lane == 0 && n_tiles > 0) {
-      mbar_expect_tx(q_full, rows_used * kD * 2);
+      mbar_expect_tx(q_full, rows_used * kDQK * 2);
 #pragma unroll
       for (int h = 0; h < Cfg::kHalves; ++h)
         tma_load_3d(q_s + h * Cfg::kSub, &tmap_q, q_full, h * 64, kvh * p.group, q0 + tq0);
@@ -130,30 +151,48 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gri
       for (int j = 0; j < n_tiles; ++j) {
         const int st = j & 1;
         const uint32_t par = ((j >> 1) & 1) ^ 1;
-        for (int kv = 0; kv < 2; ++kv) {           // kv = 0: K tile, 1: V tile
-          uint64_t* full = kv ? v_full + st : k_full + st;
-          mbar_wait(kv ? v_empty + st : k_empty + st, par);
-          mbar_expect_tx(full, kKT * kD * 2);
-          uint8_t* dst = (kv ? v_s : k_s) + st * Cfg::kKVBytes;
-          const CUtensorMap* map = kv ? &tmap_v : &tmap_k;
-          for (int i = 0; i < loads; ++i) {
-            const int t0 = (j0 + j) * kKT + i * p.box_rows;
-            int row;
-            if (p.paged) {
-              int pg = t0 / p.page_size;
-              if (pg >= n_pages) pg = n_pages - 1;    // beyond the request: masked anyway, keep the address valid
-              row = __ldg(p.kv_indices + indptr0 + pg) * p.page_size + (t0 % p.page_size);
-            } else {
-              row = kv_base + t0;
-            }
+        if constexpr (kDQK == kDV) {
+          for (int kv = 0; kv < 2; ++kv) {           // kv = 0: K tile, 1: V tile
+            uint64_t* full = kv ? v_full + st : k_full + st;
+            mbar_wait(kv ? v_empty + st : k_empty + st, par);
+            mbar_expect_tx(full, kKT * kDQK * 2);
+            uint8_t* dst = (kv ? v_s : k_s) + st * Cfg::kKBytes;
+            const CUtensorMap* map = kv ? &tmap_v : &tmap_k;
+            for (int i = 0; i < loads; ++i) {
+              const int t0 = (j0 + j) * kKT + i * p.box_rows;
+              int row;
+              if (p.paged) {
+                int pg = t0 / p.page_size;
+                if (pg >= n_pages) pg = n_pages - 1;    // beyond the request: masked anyway, keep the address valid
+                row = __ldg(p.kv_indices + indptr0 + pg) * p.page_size + (t0 % p.page_size);
+              } else {
+                row = kv_base + t0;
+              }
 #pragma unroll
-            for (int h = 0; h < Cfg::kHalves; ++h)
-              tma_load_2d(dst + h * Cfg::kSub + i * p.box_rows * 128, map, full, kvh * kD + h * 64, row);
+              for (int h = 0; h < Cfg::kHalves; ++h)
+                tma_load_2d(dst + h * Cfg::kSub + i * p.box_rows * 128, map, full, kvh * kDQK + h * 64, row);
+            }
           }
+        } else {                                     // ragged, one 128-row box per sub-tile
+          const int row = kv_base + (j0 + j) * kKT;
+          mbar_wait(k_empty + st, par);
+          mbar_expect_tx(k_full + st, kKT * kDQK * 2);
+          uint8_t* dst = k_s + st * Cfg::kKBytes;
+#pragma unroll
+          for (int h = 0; h < Cfg::kHalves - 1; ++h)     // k_nope, then the 64 k_pe columns as the last sub-tile
+            tma_load_2d(dst + h * Cfg::kSub, &tmap_k, k_full + st, kvh * kc.kv_head_stride + h * 64, row);
+          tma_load_2d(dst + (Cfg::kHalves - 1) * Cfg::kSub, &tmap_kr, k_full + st, kvh * kc.kr_head_stride, row);
+          mbar_wait(v_empty + st, par);
+          mbar_expect_tx(v_full + st, kKT * kDV * 2);
+          dst = v_s + st * Cfg::kVBytes;
+#pragma unroll
+          for (int h = 0; h < Cfg::kVHalves; ++h)
+            tma_load_2d(dst + h * Cfg::kSub, &tmap_v, v_full + st, kvh * kc.kv_head_stride + kc.v_col_off + h * 64, row);
         }
       }
     }
   } else if (warp >= 4) {
+    if constexpr (kDQK != kDV) asm volatile("setmaxnreg.inc.sync.aligned.u32 232;\n" ::: "memory");
     // ============================== consumers: S, softmax, O ==============================
     // thread (warp w of warpgroup g, lane l) holds rows rr[h] = 64 g + 16 w + l / 4 + 8 h (h = 0, 1) and columns
     // 8 j + 2 (l % 4) + e of every accumulator (tc_common.cuh fragment layout)
@@ -173,9 +212,9 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gri
     }
     const int lim_first = p.causal ? min(kv_len, tq0 + kv_off + 1) : kv_len;      // smallest limit in the tile
     float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};            // l_run: this thread's columns only
-    float o[kD / 2];
+    float o[kDV / 2];
 #pragma unroll
-    for (int i = 0; i < kD / 2; ++i) o[i] = 0.f;
+    for (int i = 0; i < kDV / 2; ++i) o[i] = 0.f;
     float s[kKT / 2];
     if (n_tiles > 0) mbar_wait(q_full, 0);
 
@@ -185,10 +224,10 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gri
       // ---- S = Q K^T ----
       mbar_wait(k_full + st, par);
       {
-        const uint32_t qa = smem_u32(q_s) + wg * 64 * 128, ka = smem_u32(k_s + st * Cfg::kKVBytes);
+        const uint32_t qa = smem_u32(q_s) + wg * 64 * 128, ka = smem_u32(k_s + st * Cfg::kKBytes);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < kD / 16; ++k) {
+        for (int k = 0; k < kDQK / 16; ++k) {
           const uint32_t off = (k >> 2) * Cfg::kSub + (k & 3) * 32;
           wgmma_bf16<kKT>(s, gmma_desc_sw128(qa + off), gmma_desc_sw128(ka + off), k > 0 ? 1u : 0u);
         }
@@ -235,7 +274,7 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gri
         l_run[h] = l_run[h] * alpha[h] + psum;
       }
 #pragma unroll
-      for (int jj = 0; jj < kD / 8; ++jj)
+      for (int jj = 0; jj < kDV / 8; ++jj)
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           o[4 * jj + 2 * h] *= alpha[h];
@@ -244,13 +283,13 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gri
       // ---- O += P V: A fragment of k step kk = S columns 16 kk .. 16 kk + 15 (rows h = 0, 1; column halves 0, 1) ----
       mbar_wait(v_full + st, par);
       {
-        const uint32_t va = smem_u32(v_s + st * Cfg::kKVBytes);
+        const uint32_t va = smem_u32(v_s + st * Cfg::kVBytes);
         wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < kKT / 16; ++kk) {
           const uint32_t a[4] = {__float_as_uint(s[8 * kk + 0]), __float_as_uint(s[8 * kk + 2]), __float_as_uint(s[8 * kk + 4]),
                                  __float_as_uint(s[8 * kk + 6])};
-          wgmma_bf16_rs_tb<kD>(o, a, gmma_desc_sw128_mn(va + kk * 2048, Cfg::kSub, 1024), 1u);
+          wgmma_bf16_rs_tb<kDV>(o, a, gmma_desc_sw128_mn(va + kk * 2048, Cfg::kSub, 1024), 1u);
         }
         wgmma_commit();
         wgmma_wait<0>();
@@ -274,17 +313,19 @@ prefill_attention_kernel(const __grid_constant__ CUtensorMap tmap_q, const __gri
         __nv_bfloat16* dst = p.o + tq * p.o_stride_n + (int64_t)head * p.o_stride_h;
         if (p.lse && (lane & 3) == 0) p.lse[tq * p.num_qo_heads + head] = lse2;
 #pragma unroll
-        for (int jj = 0; jj < kD / 8; ++jj)
+        for (int jj = 0; jj < kDV / 8; ++jj)
           *reinterpret_cast<uint32_t*>(dst + 8 * jj + cq) = pack_bf16x2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
       } else {
         const int64_t slot = ((int64_t)split * p.total_q + tq) * p.num_qo_heads + head;
-        float* pdst = p.part_o + slot * kD;
+        float* pdst = p.part_o + slot * kDV;
         if ((lane & 3) == 0) p.part_lse[slot] = lse2;
 #pragma unroll
-        for (int jj = 0; jj < kD / 8; ++jj)
+        for (int jj = 0; jj < kDV / 8; ++jj)
           *reinterpret_cast<float2*>(pdst + 8 * jj + cq) = make_float2(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
       }
     }
+  } else if constexpr (kDQK != kDV) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;\n" ::: "memory");   // warps 1..3 of warpgroup 0
   }
 }
 
@@ -312,16 +353,17 @@ prefill_merge_kernel(const PrefillParams p, int head_dim) {
   if (p.lse && threadIdx.x == 0) p.lse[tq * p.num_qo_heads + head] = wsum > 0.f ? mx + log2f(wsum) : -INFINITY;
 }
 
-template <int kD>
+template <int kDQK, int kDV>
 static int launch_prefill(const CUtensorMap& tq, const CUtensorMap& tk, const CUtensorMap& tv, const PrefillParams& p,
-                          int batch, int q_tiles, cudaStream_t stream) {
-  using Cfg = PrefillCfg<kD>;
-  constexpr auto kern = prefill_attention_kernel<kD>;
+                          int batch, int q_tiles, cudaStream_t stream, const CUtensorMap& tkr = {},
+                          const KvColumns& kc = {}) {
+  using Cfg = PrefillCfg<kDQK, kDV>;
+  constexpr auto kern = prefill_attention_kernel<kDQK, kDV>;
   XB_CUDA_OK(set_max_dynamic_smem_once<kern>(Cfg::kSmemBytes));
   dim3 grid(q_tiles, p.num_kv_heads, batch * p.kv_splits), block(kPrefillThreads);
-  XB_CUDA_OK(launch(kern, grid, block, (size_t)Cfg::kSmemBytes, stream, true, tq, tk, tv, p));
+  XB_CUDA_OK(launch(kern, grid, block, (size_t)Cfg::kSmemBytes, stream, true, tq, tk, tv, p, tkr, kc));
   if (p.kv_splits > 1)
-    XB_CUDA_OK(launch(prefill_merge_kernel, dim3((unsigned)p.total_q, p.num_qo_heads), dim3(kD < 128 ? kD : 128), 0, stream, true, p, kD));
+    XB_CUDA_OK(launch(prefill_merge_kernel, dim3((unsigned)p.total_q, p.num_qo_heads), dim3(kDV < 128 ? kDV : 128), 0, stream, true, p, kDV));
   return 0;
 }
 }  // namespace tc
@@ -391,8 +433,42 @@ static int prefill_common(const void* q, int64_t q_stride_n, int64_t q_stride_h,
   if (make_tmap_2d(&tk, k, kv_rows, (uint64_t)num_kv_heads * head_dim, (uint64_t)kv_row_stride * 2, p.box_rows, 64, 2)) return 1;
   if (make_tmap_2d(&tv, v, kv_rows, (uint64_t)num_kv_heads * head_dim, (uint64_t)kv_row_stride * 2, p.box_rows, 64, 2)) return 1;
   const int q_tiles = (max_qo_len + p.tokens_per_tile - 1) / p.tokens_per_tile;
-  return head_dim == 128 ? launch_prefill<128>(tq, tk, tv, p, batch, q_tiles, stream)
-                         : launch_prefill<64>(tq, tk, tv, p, batch, q_tiles, stream);
+  return head_dim == 128 ? launch_prefill<128, 128>(tq, tk, tv, p, batch, q_tiles, stream)
+                         : launch_prefill<64, 64>(tq, tk, tv, p, batch, q_tiles, stream);
+}
+
+// Expanded MLA prefill attention (ragged, causal, group 1, kv_splits 1): q [total_q, H, 192] (row / head strides),
+// kv_up [total_kv, H, 256] contiguous = per head [k_nope 128 | v 128], kpe [total_kv, 64] contiguous (one k_pe row per kv
+// token, shared by all heads), kv_cu_seq_lens [batch + 1] on the device; o [T, H, 128].
+int xb::mla_expanded_attention(const void* q, int64_t q_stride_n, int64_t q_stride_h, int64_t total_q, const void* kv_up,
+                               const void* kpe, int64_t total_kv, const int32_t* qo_indptr, const int32_t* kv_cu_seq_lens,
+                               void* o, int64_t o_stride_n, int64_t o_stride_h, int batch, int max_qo_len, int num_heads,
+                               float sm_scale, cudaStream_t stream) {
+  constexpr int kDQK = 192, kDV = 128, kKvW = 256;
+  if (batch == 0 || total_q == 0 || max_qo_len == 0) return 0;
+  PrefillParams p{};
+  p.qo_indptr = qo_indptr;
+  p.kv_indptr = kv_cu_seq_lens;
+  p.o = reinterpret_cast<__nv_bfloat16*>(o);
+  p.o_stride_n = o_stride_n;
+  p.o_stride_h = o_stride_h;
+  p.scale_log2 = sm_scale * 1.44269504088896340736f;
+  p.num_qo_heads = num_heads;
+  p.num_kv_heads = num_heads;
+  p.group = 1;
+  p.tokens_per_tile = 128;
+  p.causal = 1;
+  p.kv_splits = 1;
+  p.total_q = total_q;
+  p.box_rows = 128;
+  CUtensorMap tq, tk, tkr;
+  if (make_tmap_3d_bf16(&tq, q, kDQK, num_heads, total_q, (uint64_t)q_stride_h * 2, (uint64_t)q_stride_n * 2, 64, 1, 128))
+    return 1;
+  if (make_tmap_2d(&tk, kv_up, total_kv, (uint64_t)num_heads * kKvW, (uint64_t)num_heads * kKvW * 2, 128, 64, 2)) return 1;
+  if (make_tmap_2d(&tkr, kpe, total_kv, 64, 128, 128, 64, 2)) return 1;
+  const int q_tiles = (max_qo_len + 127) / 128;
+  // k_nope at column 256 h, v at 256 h + 128 of the same rows; one k_pe row for every head
+  return launch_prefill<kDQK, kDV>(tq, tk, tk, p, batch, q_tiles, stream, tkr, KvColumns{kKvW, kDV, 0});
 }
 
 extern "C" int xb_prefill_ragged_bf16(const void* q, int64_t q_stride_n, int64_t q_stride_h, const void* k, const void* v,

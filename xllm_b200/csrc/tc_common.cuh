@@ -213,4 +213,11 @@ int moe_grouped_gemm(int w4, int fc2, void* c, const void* a, const void* b, con
                      cudaStream_t stream);
 
 }  // namespace tc
+
+// expanded MLA prefill attention of mla.cu (prefill_attention.cu): ragged, causal, QK 192 = [k_nope of kv_up | shared kpe],
+// V 128 from kv_up [total_kv, H, 256]; kv_cu_seq_lens [batch + 1] on the device
+int mla_expanded_attention(const void* q, int64_t q_stride_n, int64_t q_stride_h, int64_t total_q, const void* kv_up,
+                           const void* kpe, int64_t total_kv, const int32_t* qo_indptr, const int32_t* kv_cu_seq_lens,
+                           void* o, int64_t o_stride_n, int64_t o_stride_h, int batch, int max_qo_len, int num_heads,
+                           float sm_scale, cudaStream_t stream);
 }  // namespace xb

@@ -306,6 +306,60 @@ def mla_paged_attention(plan: MlaPlan, q_nope, q_pe, ckv_cache, kpe_cache, qo_in
         _p(plan.workspace), c_i64(plan.workspace.numel()), _stream()), "mla_paged_attention")
 
 
+MLA_UP_HEAD_DIM = 256          # kv_b_proj rows per head: qk_nope_head_dim 128 | v_head_dim 128
+
+
+class MlaExpandedPlan:
+    """Host-only plan of one MLA prefill step from its host-side lengths (qo_lens: the step's q tokens, kv_lens: history +
+    the step's tokens).  `.expanded` is the form the step should take (mla_prefill_expanded when True, the absorbed
+    mla_paged_attention otherwise); `.workspace` is allocated only for the expanded form."""
+
+    def __init__(self, num_heads, qo_lens, kv_lens, device):
+        qo = (ctypes.c_int32 * len(qo_lens))(*qo_lens)
+        kv = (ctypes.c_int32 * len(kv_lens))(*kv_lens)
+        _need(len(qo_lens) == len(kv_lens), "qo_lens and kv_lens need one entry per request")
+        self.arr = (ctypes.c_int64 * 8)()
+        check(lib().xb_mla_expanded_plan(self.arr, c_i32(len(qo_lens)), c_i32(num_heads), qo, kv), "mla_expanded_plan")
+        self.expanded = bool(self.arr[0])
+        self.workspace_bytes, self.total_kv, self.num_heads = int(self.arr[1]), int(self.arr[5]), num_heads
+        self.total_q = int(self.arr[7]) & ((1 << 40) - 1)
+        self.workspace = torch.empty(self.workspace_bytes, dtype=torch.uint8, device=device) if self.expanded else None
+
+
+def mla_prefill_expanded(plan: MlaExpandedPlan, q, ckv_cache, kpe_cache, qo_indptr, paged_kv_indptr, paged_kv_indices,
+                         paged_kv_last_page_len, kv_b_proj, sm_scale: float, output, workspace=None) -> None:
+    """Expanded MLA prefill (causal): q [T, H, 192] = [q_nope | roped q_pe], caches as in mla_paged_attention, kv_b_proj
+    [H * 256, 512], output [T, H, 128] (o_proj's input).  workspace: plan.workspace unless given (at least
+    plan.workspace_bytes, layout in include/xllm_b200_ops.h)."""
+    ws = plan.workspace if workspace is None else workspace
+    _need(ws is not None, "mla_prefill_expanded: the plan chose the absorbed form and holds no workspace; pass one")
+    for t, n in ((q, "q"), (ckv_cache, "ckv_cache"), (kpe_cache, "kpe_cache"), (kv_b_proj, "kv_b_proj"), (output, "output")):
+        _cuda_bf16(t, n)
+    for t, n in ((qo_indptr, "qo_indptr"), (paged_kv_indptr, "paged_kv_indptr"), (paged_kv_indices, "paged_kv_indices"),
+                 (paged_kv_last_page_len, "paged_kv_last_page_len")):
+        _need(t.dtype == torch.int32 and t.is_cuda, f"{n} must be int32 on device")
+    H = plan.num_heads
+    _need(q.dim() == 3 and q.size(1) == H and q.size(2) == 128 + MLA_ROPE_DIM and q.stride(2) == 1,
+          f"q must be [T, {H}, 192] with contiguous rows")
+    _need(output.dim() == 3 and output.size(1) == H and output.size(2) == 128 and output.stride(2) == 1,
+          f"output must be [T, {H}, 128] with contiguous rows")
+    # the kernels read plan.total_q rows of q and write the rows qo_indptr names into output
+    _need(q.size(0) == plan.total_q and output.size(0) == plan.total_q,
+          f"q and output need the plan's {plan.total_q} tokens (got {q.size(0)} / {output.size(0)})")
+    _need(tuple(kv_b_proj.shape) == (H * MLA_UP_HEAD_DIM, MLA_KV_LORA_RANK) and kv_b_proj.is_contiguous(),
+          f"kv_b_proj must be a contiguous [{H * MLA_UP_HEAD_DIM}, {MLA_KV_LORA_RANK}] weight")
+    ckv, kpe = ckv_cache.reshape(ckv_cache.size(0), ckv_cache.size(1), -1), kpe_cache.reshape(kpe_cache.size(0), kpe_cache.size(1), -1)
+    _need(ckv.size(2) == MLA_KV_LORA_RANK and kpe.size(2) == MLA_ROPE_DIM and ckv.stride(2) == 1 and kpe.stride(2) == 1,
+          "caches must be [pages, page_size, 512] / [pages, page_size, 64] with contiguous rows")
+    _need(ws.is_cuda and ws.numel() * ws.element_size() >= plan.workspace_bytes, "workspace is smaller than the plan's")
+    check(lib().xb_mla_prefill_expanded_bf16(
+        plan.arr, _p(q), c_i64(q.stride(0)), c_i64(q.stride(1)), _p(ckv), c_i64(ckv.stride(0)), c_i64(ckv.stride(1)),
+        _p(kpe), c_i64(kpe.stride(0)), c_i64(kpe.stride(1)), c_i32(ckv.size(1)), _p(paged_kv_indptr), _p(paged_kv_indices),
+        _p(paged_kv_last_page_len), _p(qo_indptr), _p(kv_b_proj), _p(output), c_i64(output.stride(0)),
+        c_i64(output.stride(1)), c_f32(sm_scale), _p(ws), c_i64(ws.numel() * ws.element_size()), _stream()),
+        "mla_prefill_expanded")
+
+
 # ---- linears ------------------------------------------------------------------
 def matmul_small_m(a, b, bias=None, out=None):
     """xllm::kernel::cuda::matmul (cuda_ops_api.h:167-169, matmul.cpp:20-24) for M <= 64: a [M,K], b [N,K]."""
