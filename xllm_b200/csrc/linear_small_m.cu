@@ -571,8 +571,12 @@ linear_w4a16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, con
 // bf16 weights [N,K] row-major (the reference layout, untouched).
 // lane (g,t) reads rows n0+g and n0+g+8, 16 bytes each per k32 tile:
 // k in [k0+8t, k0+8t+8) -> two k16 steps (elements 0..3 -> step 0, 4..7 -> 1).
+// Warp w owns the k32 tiles w, w + 8, w + 16, ... and streams them through a per-lane private cp.async ring of
+// kBf16Ring slots in shared memory (the W4 kernel's scheme): the ring is refilled as it is consumed, so the weight
+// stream stays full until the warp's last tile.
 // ---------------------------------------------------------------------------
-template <int kMT, int kUnroll>
+constexpr int kBf16Ring = 8;
+template <int kMT>
 __global__ void __launch_bounds__(kWarps * 32)
 linear_bf16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, const __nv_bfloat16* __restrict__ x,
                            int64_t x_stride, const __nv_bfloat16* __restrict__ w,
@@ -582,9 +586,10 @@ linear_bf16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, cons
   const int g = lane >> 2, t = lane & 3;
   const int n0 = blockIdx.x * 16;
   const int ktiles = K >> 5;  // k32 tiles
-  const bool r1_ok = (n0 + g + 8) < N, r0_ok = (n0 + g) < N;
-  const __nv_bfloat16* w0 = w + (int64_t)(n0 + g) * K + 8 * t;
-  const __nv_bfloat16* w1 = w + (int64_t)(n0 + g + 8) * K + 8 * t;
+  const int nt = ktiles > warp ? (ktiles - warp + kWarps - 1) / kWarps : 0;   // tiles of this warp
+  // rows past N read row N - 1: a row of the mma's A operand only reaches its own output row, which is not stored
+  const __nv_bfloat16* w0 = w + (int64_t)min(n0 + g, N - 1) * K + 8 * t + (warp << 5);
+  const __nv_bfloat16* w1 = w + (int64_t)min(n0 + g + 8, N - 1) * K + 8 * t + (warp << 5);
 
   float acc[kMT][4];
 #pragma unroll
@@ -592,35 +597,39 @@ linear_bf16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, cons
 #pragma unroll
     for (int i = 0; i < 4; ++i) acc[m][i] = 0.f;
 
-  for (int kt0 = warp; kt0 < ktiles; kt0 += kWarps * kUnroll) {
-    uint4 wa[kUnroll], wb[kUnroll];
+  // slot = [row g chunks of the 32 lanes | row g+8 chunks]: 1 KB per warp and slot
+  extern __shared__ __align__(16) uint8_t ring_smem[];
+  const uint32_t ring = smem_addr_u32(ring_smem) + warp * (kBf16Ring * 1024) + lane * 16;
+  auto issue = [&](int j) {
+    const uint32_t dst = ring + (j & (kBf16Ring - 1)) * 1024;
+    cp_async_16(dst, w0 + (int64_t)j * (kWarps << 5));
+    cp_async_16(dst + 512, w1 + (int64_t)j * (kWarps << 5));
+  };
 #pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      const int kt = kt0 + u * kWarps;
-      wa[u] = make_uint4(0, 0, 0, 0);
-      wb[u] = make_uint4(0, 0, 0, 0);
-      if (kt < ktiles) {
-        if (r0_ok) wa[u] = ldg_stream(w0 + (kt << 5));
-        if (r1_ok) wb[u] = ldg_stream(w1 + (kt << 5));
-      }
-    }
-    if (kt0 == warp) pdl_wait();
-#pragma unroll
-    for (int u = 0; u < kUnroll; ++u) {
-      const int kt = kt0 + u * kWarps;
-      if (kt < ktiles) {
-#pragma unroll
-        for (int m = 0; m < kMT; ++m) {
-          const int tok = m * 8 + g;
-          uint4 xv = make_uint4(0, 0, 0, 0);
-          if (tok < M) xv = *reinterpret_cast<const uint4*>(x + (int64_t)tok * x_stride + (kt << 5) + 8 * t);
-          mma_bf16_16816(acc[m], wa[u].x, wb[u].x, wa[u].y, wb[u].y, xv.x, xv.y);
-          mma_bf16_16816(acc[m], wa[u].z, wb[u].z, wa[u].w, wb[u].w, xv.z, xv.w);
-        }
-      }
-    }
+  for (int j = 0; j < kBf16Ring; ++j) {
+    if (j < nt) issue(j);
+    cp_async_commit();     // one group per slot, empty or not
   }
-  if (ktiles <= warp) pdl_wait();
+  pdl_wait();  // x (and bias) come from the producer kernel
+  const __nv_bfloat16* xp[kMT];
+#pragma unroll
+  for (int m = 0; m < kMT; ++m) xp[m] = x + (int64_t)min(m * 8 + g, M - 1) * x_stride + 8 * t + (warp << 5);
+#pragma unroll 1
+  for (int j = 0; j < nt; ++j) {
+    cp_async_wait<kBf16Ring - 1>();
+    const uint32_t src = ring + (j & (kBf16Ring - 1)) * 1024;
+    const uint4 wa = lds_128(src), wb = lds_128(src + 512);
+#pragma unroll
+    for (int m = 0; m < kMT; ++m) {
+      uint4 xv = *reinterpret_cast<const uint4*>(xp[m] + (int64_t)j * (kWarps << 5));
+      if (m * 8 + g >= M) xv = make_uint4(0, 0, 0, 0);
+      mma_bf16_16816(acc[m], wa.x, wb.x, wa.y, wb.y, xv.x, xv.y);
+      mma_bf16_16816(acc[m], wa.z, wb.z, wa.w, wb.w, xv.z, xv.w);
+    }
+    // the LDS of this slot have returned before the HMMAs that use them issue: the refill cannot overtake them
+    if (j + kBf16Ring < nt) issue(j + kBf16Ring);
+    cp_async_commit();
+  }
   pdl_launch_dependents();
 
 #pragma unroll
@@ -694,14 +703,51 @@ struct W4Launch {
   bool tg2, xs, exact;
 };
 
+// What padding the shared memory of a W4 launch needs: the CTAs of `kern` an SM holds at `smem` bytes of dynamic shared
+// memory, the kernel's static shared memory and the device's per-SM / per-CTA-reserved shared memory.  Also lets the
+// kernel take up to half an SM's shared memory dynamically.
+struct W4Residency {
+  cudaError_t err;
+  int resident, static_smem, smem_per_sm, reserved_per_cta;
+};
+template <typename K>
+static W4Residency w4_residency(K kern, int smem) {
+  W4Residency r{cudaSuccess, 0, 0, 0, 0};
+  cudaFuncAttributes fa{};
+  int dev = 0;
+  if ((r.err = cudaGetDevice(&dev)) != cudaSuccess ||
+      (r.err = cudaDeviceGetAttribute(&r.smem_per_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev)) != cudaSuccess ||
+      (r.err = cudaDeviceGetAttribute(&r.reserved_per_cta, cudaDevAttrReservedSharedMemoryPerBlock, dev)) != cudaSuccess ||
+      (r.err = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, r.smem_per_sm / 2)) != cudaSuccess ||
+      (r.err = cudaFuncGetAttributes(&fa, kern)) != cudaSuccess ||
+      (r.err = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&r.resident, kern, kWarps * 32, smem)) != cudaSuccess)
+    return r;
+  r.static_smem = (int)fa.sharedSizeBytes;
+  return r;
+}
+
 template <int kMT, int kSplit, int kTG, int kEpi, bool kXs, bool kExact>
 static int w4_launch(const W4Launch& l) {
   constexpr int kDepth = kW4RingTiles / kTG;
   constexpr auto kern = linear_w4a16_small_m_kernel<kMT, kSplit, kDepth, kTG, 2, kEpi, kXs, kExact>;
-  // static reduction scratch + ring (+ x stage) may exceed the default 48 KB
-  XB_CUDA_OK(set_max_dynamic_smem_once<kern>((int)(w4_ring_bytes(kDepth, kTG) + (kXs ? kXsMaxBytes : 0))));
   const dim3 grid((l.N / 16 + kWarps / kSplit - 1) / (kWarps / kSplit)), block(kWarps * 32);
-  XB_CUDA_OK(launch(kern, grid, block, w4_ring_bytes(kDepth, kTG) + l.xs_bytes, l.stream, true, l.y, l.y_stride, l.x,
+  size_t smem = w4_ring_bytes(kDepth, kTG) + l.xs_bytes;
+  if constexpr (kXs) {
+    // static reduction scratch + ring + x stage may exceed the default 48 KB
+    XB_CUDA_OK(set_max_dynamic_smem_once<kern>((int)(w4_ring_bytes(kDepth, kTG) + kXsMaxBytes)));
+  } else {
+    // The block scheduler does not spread a one-wave grid evenly when SMs have room for more CTAs than the even share:
+    // o_proj / down_proj of Qwen2-7B (224 CTAs on 132 SMs that hold 3 each) stream like SMs holding 3 CTAs.  Padding
+    // the shared memory so that an SM holds at most ceil(grid / SMs) CTAs took down_proj from 18.0 to 15.9 us (H100).
+    // The carveout preference is left to the driver: forcing the maximum shared carveout as well measured 445 instead
+    // of 459 decode tokens/s.
+    static const W4Residency res = w4_residency(kern, (int)smem);
+    XB_CUDA_OK(res.err);
+    const int per_sm = ((int)grid.x + device_sm_count() - 1) / device_sm_count();
+    if (per_sm < res.resident)
+      smem = std::max(smem, (size_t)(res.smem_per_sm / (per_sm + 1) + 128 - res.reserved_per_cta - res.static_smem));
+  }
+  XB_CUDA_OK(launch(kern, grid, block, smem, l.stream, true, l.y, l.y_stride, l.x,
                     l.x_stride, l.qw, l.meta, l.bias, l.M, l.N, l.K, l.gshift, l.act_mode, l.fz));
   return 0;
 }
@@ -867,6 +913,17 @@ extern "C" int xb_linear_w4a16_decode_fused_fits(int M, int K) {
   return M >= 1 && M <= 8 && w4_xs_bytes(M, K) <= kXsMaxBytes ? 1 : 0;
 }
 
+template <int kMT>
+static int bf16_small_m_launch(__nv_bfloat16* y, int64_t y_stride, const __nv_bfloat16* x, int64_t x_stride,
+                               const __nv_bfloat16* w, const __nv_bfloat16* bias, int M, int N, int K, cudaStream_t s) {
+  constexpr auto kern = linear_bf16_small_m_kernel<kMT>;
+  constexpr int kRingBytes = kWarps * kBf16Ring * 1024;
+  XB_CUDA_OK(set_max_dynamic_smem_once<kern>(kRingBytes));
+  XB_CUDA_OK(launch(kern, dim3((N + 15) / 16), dim3(kWarps * 32), kRingBytes, s, true, y, y_stride, x, x_stride, w, bias,
+                    M, N, K));
+  return 0;
+}
+
 extern "C" int xb_linear_bf16_small_m(void* y, int64_t y_stride, const void* x, int64_t x_stride, const void* w,
                                       const void* bias, int M, int N, int K, xb_stream_t stream) {
   if (M == 0) return 0;
@@ -879,16 +936,10 @@ extern "C" int xb_linear_bf16_small_m(void* y, int64_t y_stride, const void* x, 
   auto* xx = reinterpret_cast<const __nv_bfloat16*>(x);
   auto* ww = reinterpret_cast<const __nv_bfloat16*>(w);
   auto* bb = reinterpret_cast<const __nv_bfloat16*>(bias);
-  dim3 grid((N + 15) / 16), block(kWarps * 32);
-  cudaStream_t s = (cudaStream_t)stream;
-#define XB_BF(MT, U) \
-  XB_CUDA_OK(launch(linear_bf16_small_m_kernel<MT, U>, grid, block, 0, s, true, yy, y_stride, xx, x_stride, ww, bb, M, N, K))
-  if (M <= 8) XB_BF(1, 8);
-  else if (M <= 16) XB_BF(2, 4);
-  else if (M <= 32) XB_BF(4, 2);
-  else XB_BF(8, 1);
-#undef XB_BF
-  return 0;
+  if (M <= 8) return bf16_small_m_launch<1>(yy, y_stride, xx, x_stride, ww, bb, M, N, K, (cudaStream_t)stream);
+  if (M <= 16) return bf16_small_m_launch<2>(yy, y_stride, xx, x_stride, ww, bb, M, N, K, (cudaStream_t)stream);
+  if (M <= 32) return bf16_small_m_launch<4>(yy, y_stride, xx, x_stride, ww, bb, M, N, K, (cudaStream_t)stream);
+  return bf16_small_m_launch<8>(yy, y_stride, xx, x_stride, ww, bb, M, N, K, (cudaStream_t)stream);
 }
 
 // Host-side packer (plain C++): q[N,K] (one 4-bit value per byte) -> tile layout.
