@@ -78,10 +78,10 @@ def _w4(N, K, gs, seed, bias):
 @pytest.mark.parametrize("nh,nkv,D,K", [(28, 4, 128, 3584), (14, 2, 64, 896), (8, 1, 128, 8192)])
 @pytest.mark.parametrize("M", [1, 3, 8])
 @pytest.mark.parametrize("staged", [False, True])
-def test_fused_rope_epilogue_equals_gemv_then_rope(M, nh, nkv, D, K, staged, built_lib, oracle_form="bf16w"):
+def test_fused_rope_epilogue_equals_gemv_then_rope(M, nh, nkv, D, K, staged, built_lib, oracle_form="bf16w", gs=None):
     from xllm_b200 import ops, quant
     N = (nh + 2 * nkv) * D
-    gs = 128 if K % 128 == 0 else 64
+    gs = gs or (128 if K % 128 == 0 else 64)
     if staged and not ops.w4a16_decode_fused_fits(M, K):
         pytest.skip("activation block does not fit the shared-memory stage (the runner falls back to the unstaged kernel)")
     q, s, z, b = _w4(N, K, gs, 11, bias=True)
@@ -120,13 +120,13 @@ def test_fused_rope_epilogue_equals_gemv_then_rope(M, nh, nkv, D, K, staged, bui
 @pytest.mark.parametrize("N,K,epi", [(4608, 3584, "none"), (37888, 3584, "act_mul"), (1024, 8192, "none"), (2432, 896, "none")])
 @pytest.mark.parametrize("M", [1, 4, 8])
 @pytest.mark.parametrize("with_res", [True, False])
-def test_fused_norm_prologue(M, N, K, epi, with_res, built_lib):
+def test_fused_norm_prologue(M, N, K, epi, with_res, built_lib, gs=None):
     from xllm_b200 import ops, quant
     if M * (K + 8) * 2 + 256 > 72 * 1024:
         assert not ops.w4a16_decode_fused_fits(M, K)
         pytest.skip("activation block does not fit the shared-memory stage (the runner falls back to separate launches)")
     assert ops.w4a16_decode_fused_fits(M, K)
-    gs = 128 if K % 128 == 0 else 64
+    gs = gs or (128 if K % 128 == 0 else 64)
     q, s, z, b = _w4(N, K, gs, 21, bias=(N == 4608))
     g = torch.Generator().manual_seed(31)
     x = torch.randn(M, K, generator=g).to(BF16)
@@ -162,10 +162,9 @@ def test_fused_norm_prologue(M, N, K, epi, with_res, built_lib):
 
 
 @pytest.mark.parametrize("N,K", [(3584, 3584), (3584, 18944), (37888, 3584)])
-def test_staged_x_is_bit_identical(N, K, built_lib):
+def test_staged_x_is_bit_identical(N, K, built_lib, gs=128):
     from xllm_b200 import ops
     g = torch.Generator(device=DEV).manual_seed(1)
-    gs = 128
     qw = torch.randint(-2 ** 31, 2 ** 31 - 1, (N // 16, K // 64, 32, 4), generator=g, device=DEV, dtype=torch.int32)
     sc = (torch.rand(K // gs, N, generator=g, device=DEV) * 0.01 + 0.001).to(BF16).view(torch.int16).to(torch.int32) & 0xFFFF
     meta = (sc | (0x4308 << 16)).contiguous()
@@ -182,7 +181,7 @@ def test_staged_x_is_bit_identical(N, K, built_lib):
 @pytest.mark.parametrize("H,Kin,Nout,epi", [(3584, 3584, 4608, "none"), (3584, 18944, 37888, "act_mul"), (896, 896, 1152, "none"),
                                             (8192, 8192, 1280, "none")])
 @pytest.mark.parametrize("M", [1, 3, 8])
-def test_split_rms_norm_producer_and_consumer(M, H, Kin, Nout, epi, built_lib):
+def test_split_rms_norm_producer_and_consumer(M, H, Kin, Nout, epi, built_lib, gs=None):
     """RMSNorm split over two linears: the row-parallel projection (producer, epilogue "residual_stats") adds the
     residual and emits the updated residual stream + per-tile partial sums of its squares; the next linear (consumer,
     norm_stats_in) normalises that stream while staging it.  Checked against fused_add_rms_norm -> linear of the oracle:
@@ -191,7 +190,7 @@ def test_split_rms_norm_producer_and_consumer(M, H, Kin, Nout, epi, built_lib):
     from xllm_b200 import ops, quant
     if not ops.w4a16_decode_fused_fits(M, H):
         pytest.skip("the consumer's activation block does not fit the shared-memory stage")
-    gs = 128 if Kin % 128 == 0 and H % 128 == 0 else 64
+    gs = gs or (128 if Kin % 128 == 0 and H % 128 == 0 else 64)
     g = torch.Generator().manual_seed(41)
     q1, s1, z1, _ = _w4(H, Kin, gs, 5, bias=False)               # producer: [H, Kin] (o_proj / down_proj)
     q2, s2, z2, b2 = _w4(Nout, H, gs, 6, bias=(Nout == 4608))    # consumer: [Nout, H] (qkv / gate_up)

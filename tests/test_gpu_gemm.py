@@ -4,6 +4,7 @@ import torch
 
 from oracle import ops as O
 from oracle import quant as Q
+from tests.group_probe import group_probe_weights
 from tests.util import assert_close_bf16, assert_close_sum
 
 pytestmark = pytest.mark.gpu
@@ -140,17 +141,17 @@ def test_gemm_w4a16(M, N, K, built_lib):
 
 
 def test_gemm_w4a16_dequant_bit_exact(built_lib):
-    """identity activations read the dequantised weights back out of the tensor-core path bit-for-bit."""
+    """identity activations read the dequantised weights back out of the tensor-core path bit-for-bit, at every group size
+    from 64 to K; scales and zeros differ from group to group, so a k block that reads another group's meta row shows."""
     from xllm_b200 import ops, quant
-    g = torch.Generator().manual_seed(11)
-    N, K, gs = 256, 256, 128
-    w = torch.randn(N, K, generator=g).to(BF16)
-    q, s, z = Q.quantize(w, 4, gs)
-    wd = Q.dequantize(q, s, z, gs)
-    qw, meta = quant.pack_w4(q, s, z, gs)
-    x = torch.eye(K, dtype=BF16)
-    y = ops.gemm_w4a16(x.to(DEV), qw.to(DEV), meta.to(DEV), gs)
-    assert torch.equal(y.cpu(), wd.t().contiguous())
+    N, K = 256, 2048
+    x = torch.eye(K, dtype=BF16, device=DEV)
+    for gs in (64, 128, 256, 512, K):
+        q, s, z = group_probe_weights(N, K, gs, 4, seed=11)
+        wd = Q.dequantize(q, s, z, gs)
+        qw, meta = quant.pack_w4(q, s, z, gs)
+        y = ops.gemm_w4a16(x, qw.to(DEV), meta.to(DEV), gs)
+        assert torch.equal(y.cpu(), wd.t().contiguous()), f"dequant mismatch at group size {gs}"
 
 
 def test_w4a16_decode_and_prefill_kernels_agree(built_lib):

@@ -4,6 +4,7 @@ import torch
 
 from oracle import ops as O
 from oracle import quant as Q
+from tests.group_probe import PROBE_K, w4_probe
 from tests.util import assert_close_bf16, assert_close_sum
 
 
@@ -68,19 +69,9 @@ def test_linear_w4a16_small_m(M, N, K, sym, built_lib):
 
 def test_w4a16_dequant_is_bit_exact(built_lib):
     """x = identity rows picks out single weights: y[m, n] = bf16(w[n, k_m]) must equal the spec's dequantised
-    weight bit-for-bit (one rounding in (q-z)*s)."""
-    from xllm_b200 import ops, quant
-    g = torch.Generator().manual_seed(11)
-    N, K, gs = 64, 256, 128
-    w = torch.randn(N, K, generator=g).to(BF16)
-    q, s, z = Q.quantize(w, 4, gs)
-    wd = Q.dequantize(q, s, z, gs)
-    qw, meta = quant.pack_w4(q, s, z, gs)
-    for k0 in range(0, K, 64):
-        x = torch.zeros(64, K, dtype=BF16)
-        x[torch.arange(64), k0 + torch.arange(64)] = 1.0
-        y = ops.w4a16_linear_small_m(x.to(DEV), qw.to(DEV), meta.to(DEV), gs)
-        assert torch.equal(y.cpu(), wd[:, k0:k0 + 64].t().contiguous()), f"dequant mismatch in k block {k0}"
+    weight bit-for-bit (one rounding in (q-z)*s), at every group size from 64 to K (tests/group_probe.py)."""
+    for gs in (64, 128, 256, 512, PROBE_K):
+        w4_probe(gs)
 
 
 def test_linear_linearity_full_size(built_lib):

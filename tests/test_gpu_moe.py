@@ -90,7 +90,8 @@ def test_fused_moe_layer(built_lib):
     assert_close_bf16(y, ref, ulps=6, rel_l2=5e-3, what="FusedMoE layer", atol=2.0 ** -9)
 
 
-@pytest.mark.parametrize("T,k,E,H,I,gs", [(1, 2, 4, 256, 128, 64), (4, 8, 32, 1024, 512, 128), (3, 6, 16, 2048, 1408, 128)])
+@pytest.mark.parametrize("T,k,E,H,I,gs", [(1, 2, 4, 256, 128, 64), (4, 8, 32, 1024, 512, 128), (3, 6, 16, 2048, 1408, 128),
+                                            (3, 4, 8, 1024, 512, 256), (64, 2, 4, 512, 512, 512), (2, 2, 4, 2048, 1024, 1024)])
 def test_fused_moe_w4a16_decode(T, k, E, H, I, gs, built_lib):
     """W4A16 experts (additive, BASELINE configs[4]): per-expert tile-packed int4 weights through the expert-indexed GEMVs vs the
     oracle MoE on the dequantised weights (spec form 1 of oracle/quant.py: w = bf16((q - z) s))."""

@@ -128,7 +128,8 @@ def test_grouped_bf16(T, E, k, H, I, built_lib):
 
 
 @pytest.mark.parametrize("T", [65, 256, 1000])
-@pytest.mark.parametrize("E,k,H,I,gs", [(8, 2, 512, 128, 64), (8, 4, 512, 1408, 128), (4, 2, 7168, 128, 128)])
+@pytest.mark.parametrize("E,k,H,I,gs", [(8, 2, 512, 128, 64), (8, 4, 512, 1408, 128), (4, 2, 7168, 128, 128), (8, 2, 1024, 512, 256),
+                                         (4, 2, 512, 512, 512)])
 def test_grouped_w4a16(T, E, k, H, I, gs, built_lib):
     g, x, w = _problem("w4", T * 37 + E, T, k, E, H, I, gs)
     ids = _random_ids(g, T, k, E)

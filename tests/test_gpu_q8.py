@@ -5,6 +5,7 @@ import torch
 
 from oracle import ops as O
 from oracle import quant as Q
+from tests.group_probe import group_probe_weights
 from tests.util import assert_close_bf16, assert_close_sum
 
 pytestmark = pytest.mark.gpu
@@ -43,26 +44,24 @@ def test_linear_w8a16_small_m(M, N, K, sym, built_lib):
 
 def test_w8a16_dequant_is_bit_exact(built_lib):
     """identity activations read single weights back: every one of the 256 levels, zero points across the 8-bit range
-    and both kernels (streaming and wgmma converter) must reproduce bf16((q - z) * s) bit for bit."""
+    and both kernels (streaming and wgmma converter) must reproduce bf16((q - z) * s) bit for bit, at every group size from
+    64 to K; scales and zeros differ from group to group, so reading another group's meta row shows."""
     from xllm_b200 import ops, quant
-    g = torch.Generator().manual_seed(11)
-    N, K, gs = 256, 256, 128
-    q = torch.randint(0, 256, (N, K), dtype=torch.uint8, generator=g)
-    q[0, :256] = torch.arange(256, dtype=torch.uint8)                  # all levels in one row
-    s = (torch.rand(N, K // gs, generator=g) * 0.01 + 0.001).to(BF16)
-    z = torch.randint(0, 256, (N, K // gs), dtype=torch.uint8, generator=g)
-    z[0, 0], z[0, 1], z[1, 0], z[1, 1] = 0, 255, 128, 127
-    wd = Q.dequantize(q, s, z, gs)
-    qw, meta = quant.pack_w8(q, s, z, gs)
-    assert torch.equal(qw, quant.pack_w8_c(q)), "torch and C packers disagree"
-    qw, meta = qw.to(DEV), meta.to(DEV)
-    for k0 in range(0, K, 64):
-        x = torch.zeros(64, K, dtype=BF16)
-        x[torch.arange(64), k0 + torch.arange(64)] = 1.0
-        y = ops.w8a16_linear_small_m(x.to(DEV), qw, meta, gs)
-        assert torch.equal(y.cpu(), wd[:, k0:k0 + 64].t().contiguous()), f"streaming kernel: dequant mismatch in k block {k0}"
-    y = ops.gemm_w8a16(torch.eye(K, dtype=BF16).to(DEV), qw, meta, gs)
-    assert torch.equal(y.cpu(), wd.t().contiguous()), "wgmma converter: dequant mismatch"
+    N, K = 256, 2048
+    eye = torch.eye(K, dtype=BF16, device=DEV)
+    for gs in (64, 128, 256, 512, K):
+        q, s, z = group_probe_weights(N, K, gs, 8, seed=11)             # zero points (n + 7 g) mod 256: the whole range
+        q[0, :256] = torch.arange(256, dtype=torch.uint8)              # all levels in one row
+        wd = Q.dequantize(q, s, z, gs)
+        qw, meta = quant.pack_w8(q, s, z, gs)
+        assert torch.equal(qw, quant.pack_w8_c(q)), "torch and C packers disagree"
+        qw, meta = qw.to(DEV), meta.to(DEV)
+        for k0 in range(0, K, 64):
+            y = ops.w8a16_linear_small_m(eye[k0:k0 + 64], qw, meta, gs)
+            assert torch.equal(y.cpu(), wd[:, k0:k0 + 64].t().contiguous()), \
+                f"streaming kernel: dequant mismatch in k block {k0} at group size {gs}"
+        y = ops.gemm_w8a16(eye, qw, meta, gs)
+        assert torch.equal(y.cpu(), wd.t().contiguous()), f"wgmma converter: dequant mismatch at group size {gs}"
 
 
 @pytest.mark.parametrize("M,N,K", [(128, 4608, 3584), (333, 3584, 3584), (2048, 37888, 3584), (512, 3584, 18944), (17, 1152, 896),

@@ -836,9 +836,10 @@ extern "C" int xb_gemm_w4a16(void* c, int64_t ldc, const void* a, int64_t lda, c
                              const void* bias, int M, int N, int K, int group_size, xb_stream_t stream) {
   if (M == 0 || N == 0) return 0;
   XB_CHECK(N % 64 == 0 && K % 64 == 0, "gemm_w4a16: N=%d and K=%d must be multiples of 64", N, K);
-  XB_CHECK(group_size >= 64 && K % group_size == 0, "gemm_w4a16: bad group_size %d", group_size);
+  XB_CHECK(group_size >= 64 && group_size % 64 == 0 && K % group_size == 0,
+           "gemm_w4a16: group_size %d must be a multiple of 64 dividing K=%d", group_size, K);
   const int tpg = group_size / 64;
-  XB_CHECK((tpg & (tpg - 1)) == 0, "gemm_w4a16: group_size/64 must be a power of two");
+  XB_CHECK((tpg & (tpg - 1)) == 0, "gemm_w4a16: group_size/64 must be a power of two (got %d)", group_size);
   XB_CHECK(lda % 8 == 0 && (reinterpret_cast<uintptr_t>(a) & 15) == 0, "gemm_w4a16: a alignment");
   GemmParams p{};
   p.c = reinterpret_cast<__nv_bfloat16*>(c);
@@ -867,9 +868,10 @@ extern "C" int xb_gemm_w8a16(void* c, int64_t ldc, const void* a, int64_t lda, c
                              const void* bias, int M, int N, int K, int group_size, xb_stream_t stream) {
   if (M == 0 || N == 0) return 0;
   XB_CHECK(N % 64 == 0 && K % 64 == 0, "gemm_w8a16: N=%d and K=%d must be multiples of 64", N, K);
-  XB_CHECK(group_size >= 64 && K % group_size == 0, "gemm_w8a16: bad group_size %d", group_size);
+  XB_CHECK(group_size >= 64 && group_size % 64 == 0 && K % group_size == 0,
+           "gemm_w8a16: group_size %d must be a multiple of 64 dividing K=%d", group_size, K);
   const int tpg = group_size / 64;
-  XB_CHECK((tpg & (tpg - 1)) == 0, "gemm_w8a16: group_size/64 must be a power of two");
+  XB_CHECK((tpg & (tpg - 1)) == 0, "gemm_w8a16: group_size/64 must be a power of two (got %d)", group_size);
   XB_CHECK(lda % 8 == 0 && (reinterpret_cast<uintptr_t>(a) & 15) == 0, "gemm_w8a16: a alignment");
   GemmParams p{};
   p.c = reinterpret_cast<__nv_bfloat16*>(c);

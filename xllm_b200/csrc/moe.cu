@@ -652,7 +652,7 @@ extern "C" int xb_moe_experts_w4a16(void* out, int64_t out_stride, const void* i
   XB_CHECK(group_size >= 64 && group_size % 64 == 0 && hidden % group_size == 0 && inter % group_size == 0,
            "moe_experts_w4a16: group_size %d must be a multiple of 64 dividing hidden and inter", group_size);
   const int tpg = group_size / 64;
-  XB_CHECK((tpg & (tpg - 1)) == 0, "moe_experts_w4a16: group_size / 64 must be a power of two");
+  XB_CHECK((tpg & (tpg - 1)) == 0, "moe_experts_w4a16: group_size / 64 must be a power of two (got %d)", group_size);
   int gshift = 0;
   while ((1 << gshift) < tpg) ++gshift;
   const MoeLayout l = moe_layout(num_tokens, topk, hidden, inter);
