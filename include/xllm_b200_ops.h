@@ -189,6 +189,9 @@ int xb_debug_set_decode_trace(void* buf);
 /* debug aid: number of thread-block clusters of `cluster` CTAs of the paged decode kernel the current device can run
  * concurrently (cudaOccupancyMaxActiveClusters), -1 if that cluster size cannot be launched. */
 int xb_debug_max_active_clusters(int cluster);
+/* debug aid: cluster size the most recent xb_paged_decode_bf16 launch of this process used (1 when the launcher fell
+ * back from the planned size because the device cannot co-schedule it), 0 before the first launch. */
+int xb_debug_last_decode_cluster(void);
 int xb_paged_decode_bf16(const int64_t* plan8, const void* q, int64_t q_stride_n,
                          int64_t q_stride_h, const void* k_cache,
                          const void* v_cache, int64_t kv_stride_page,

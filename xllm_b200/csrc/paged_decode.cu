@@ -550,6 +550,7 @@ paged_decode_kernel(const DecodeParams p) {
 
 namespace {
 unsigned long long* g_decode_trace = nullptr;   // debug only (xb_debug_set_decode_trace)
+std::atomic<int> g_last_decode_cluster{0};       // debug only (xb_debug_last_decode_cluster)
 }
 
 template <int kD, int kGT, int kW>
@@ -586,6 +587,7 @@ static int launch_decode_w(DecodeParams& p, int batch, int splits, cudaStream_t 
   }();
   // the plan's cluster size is a request: fall back to per-CTA partials (cluster 1) when the device cannot co-schedule it
   if (p.cluster > max_cluster || splits % p.cluster != 0) p.cluster = 1;
+  g_last_decode_cluster.store(p.cluster, std::memory_order_relaxed);
   p.trace = g_decode_trace;
   dim3 grid(splits, p.num_kv_heads * p.head_tiles, batch), block(kW * 32);
   XB_CUDA_OK(launch_cluster(kern, grid, block, smem, stream, true, p.cluster, p));
@@ -765,6 +767,10 @@ extern "C" int xb_debug_max_active_clusters(int cluster) {
   }
   return n;
 }
+
+// debug: cluster size (CTAs along the split axis) of the most recent paged_decode launch of this process, after the
+// fall-back to 1 when the device cannot co-schedule the planned size; 0 before the first launch.
+extern "C" int xb_debug_last_decode_cluster() { return g_last_decode_cluster.load(std::memory_order_relaxed); }
 
 // debug: per-CTA stage timestamps (%globaltimer, ns) of the next paged_decode launches: buf = uint64[ctas][8], or null.
 extern "C" int xb_debug_set_decode_trace(void* buf) {

@@ -209,6 +209,9 @@ class DecodePlan:
         self.arr = (ctypes.c_int64 * 8)()
         check(lib().xb_decode_plan(self.arr, c_i32(batch), c_i32(num_qo_heads), c_i32(num_kv_heads), c_i32(head_dim),
                                    c_i32(page_size), c_i32(max_pages_per_request), c_i32(num_sms)), "decode_plan")
+        # the shapes batch_decode's tensors must have: query / output, and a cache without its block dimension
+        self.q_shape = (batch, num_qo_heads, head_dim)
+        self.page_shape = (page_size, num_kv_heads, head_dim)
         # chunk_tokens: nominal split size at the planned maximum context (the kernel derives the live one on the device);
         # max_splits: splits launched per (request, kv head) = clusters x cluster size
         self.chunk_tokens, self.max_splits = int(self.arr[0]), int(self.arr[1])
@@ -228,10 +231,24 @@ def batch_decode(plan: DecodePlan, query, k_cache, v_cache, paged_kv_indptr, pag
     for t, n in ((paged_kv_indptr, "paged_kv_indptr"), (paged_kv_indices, "paged_kv_indices"),
                  (paged_kv_last_page_len, "paged_kv_last_page_len")):
         _need(t.dtype == torch.int32 and t.is_cuda, f"{n} must be int32 on device")
-    _need(query.dim() == 3 and k_cache.dim() == 4, "query [B,Hq,D], caches [blocks,page,Hkv,D]")
+    # The kernel takes the plan's geometry and one set of strides for both caches: anything else would be read with the
+    # wrong layout, or past the end of a tensor, without an error.  (Messages are formatted only on failure: this runs
+    # once per layer and step.)
+    if query.shape != plan.q_shape or output.shape != plan.q_shape:
+        raise XllmB200Error(f"query {tuple(query.shape)} and output {tuple(output.shape)} must be "
+                            f"[batch, num_qo_heads, head_dim] = {list(plan.q_shape)} of the plan")
+    if k_cache.shape[1:] != plan.page_shape or v_cache.shape != k_cache.shape:
+        raise XllmB200Error(f"k_cache {tuple(k_cache.shape)} and v_cache {tuple(v_cache.shape)} must be [blocks, page_size, "
+                            f"num_kv_heads, head_dim] with [page_size, num_kv_heads, head_dim] = {list(plan.page_shape)} "
+                            "of the plan")
+    kv_stride = k_cache.stride()
+    if v_cache.stride() != kv_stride:
+        raise XllmB200Error(f"v_cache strides {v_cache.stride()} differ from k_cache strides {kv_stride}")
+    _need(query.stride(2) == 1 and output.stride(2) == 1 and kv_stride[3] == 1,
+          "the last dimension of query, output and the caches must be unit-stride")
     check(lib().xb_paged_decode_bf16(plan.arr, _p(query), c_i64(query.stride(0)), c_i64(query.stride(1)), _p(k_cache),
-                                     _p(v_cache), c_i64(k_cache.stride(0)), c_i64(k_cache.stride(1)),
-                                     c_i64(k_cache.stride(2)), _p(paged_kv_indptr), _p(paged_kv_indices),
+                                     _p(v_cache), c_i64(kv_stride[0]), c_i64(kv_stride[1]),
+                                     c_i64(kv_stride[2]), _p(paged_kv_indptr), _p(paged_kv_indices),
                                      _p(paged_kv_last_page_len), _p(output), c_i64(output.stride(0)),
                                      c_i64(output.stride(1)), _p(output_lse), c_f32(sm_scale), _p(plan.float_ws),
                                      _p(plan.int_ws), _stream()), "batch_decode")
