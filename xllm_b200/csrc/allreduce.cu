@@ -131,7 +131,8 @@ allreduce_add_rms_norm_kernel(__nv_bfloat16* __restrict__ out, __nv_bfloat16* __
       zr[k] = z;
     }
   }
-  // block sum
+  // the residual add, squares and block sum above are add_bf16x8 / sumsq_bf16x8 / block_sum written out on the fp32
+  // all-reduce sums: through the helpers this kernel, which no single-GPU test runs, compiles to different code
   ss = warp_sum(ss);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
   __syncthreads();
@@ -141,20 +142,13 @@ allreduce_add_rms_norm_kernel(__nv_bfloat16* __restrict__ out, __nv_bfloat16* __
     if (threadIdx.x == 0) red[32] = t;
   }
   __syncthreads();
-  const float rstd = rsqrtf(red[32] / (float)hidden + eps);
+  const float rstd = rms_rstd(red[32], hidden, eps);
 #pragma unroll
   for (int k = 0; k < kMaxVec; ++k) {
     const int idx = threadIdx.x + k * blockDim.x;
     if (idx < nvec) {
-      const uint4 w = __ldg(reinterpret_cast<const uint4*>(weight) + idx);
-      const uint32_t* zp = &zr[k].x;
-      const uint32_t* wp = &w.x;
-      uint4 o;
-      uint32_t* op = &o.x;
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        op[j] = pack_bf16x2(round_bf16(bf16lo(zp[j]) * rstd) * bf16lo(wp[j]), round_bf16(bf16hi(zp[j]) * rstd) * bf16hi(wp[j]));
-      reinterpret_cast<uint4*>(out + tok * hidden)[idx] = o;
+      reinterpret_cast<uint4*>(out + tok * hidden)[idx] =
+          rms_apply_bf16x8(zr[k], __ldg(reinterpret_cast<const uint4*>(weight) + idx), rstd);
     }
   }
 }

@@ -279,5 +279,159 @@ __device__ __forceinline__ void store_c_frag(float* tile16x8, const float (&c)[4
   tile16x8[(g + 8) * 8 + 2 * t + 1] = c[3];
 }
 
+// ---- reference arithmetic ---------------------------------------------------
+// The rounding order of the reference's RMSNorm (xllm/core/kernels/cuda/norm.cu), RoPE (rope.cu) and gated activations
+// (activation.cu).  Every kernel that normalises, rotates or gates a row calls these, which keeps the fused forms
+// bit-identical to the unfused kernels.
+
+// block-wide sum (<= 1024 threads, smem[33]); stands in for the cub::BlockReduce of norm.cu:60-62
+__device__ __forceinline__ float block_sum(float v, float* smem) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  v = warp_sum(v);
+  if (lane == 0) smem[warp] = v;
+  __syncthreads();
+  const int nwarps = (blockDim.x + 31) >> 5;
+  if (warp == 0) {
+    float t = lane < nwarps ? smem[lane] : 0.f;
+    t = warp_sum(t);
+    if (lane == 0) smem[32] = t;
+  }
+  __syncthreads();
+  return smem[32];
+}
+
+// bf16 residual add, one rounding per element (norm.cu:112, _f16Vec::operator+= of type_convert.cuh:150-169)
+__device__ __forceinline__ float add_bf16(float x, float r) {
+  return round_bf16(x + r);
+}
+__device__ __forceinline__ uint4 add_bf16x8(const uint4 x, const uint4 r) {
+  const uint32_t* xp = &x.x;
+  const uint32_t* rp = &r.x;
+  uint4 o;
+  uint32_t* op = &o.x;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) op[j] = pack_bf16x2(bf16lo(xp[j]) + bf16lo(rp[j]), bf16hi(xp[j]) + bf16hi(rp[j]));
+  return o;
+}
+
+// ss + sum of squares of the 8 bf16 of x, fp32 in element order (_f16Vec::sum_squares, type_convert.cuh:213-228)
+__device__ __forceinline__ float sumsq_bf16x8(float ss, const uint4 x) {
+  const uint32_t* xp = &x.x;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    float a = bf16lo(xp[j]), b = bf16hi(xp[j]);
+    ss += a * a + b * b;
+  }
+  return ss;
+}
+
+// 1 / RMS of a row of n elements from its sum of squares (norm.cu:65,122)
+__device__ __forceinline__ float rms_rstd(float sumsq, int n, float eps) {
+  return rsqrtf(sumsq / (float)n + eps);
+}
+
+// normalised value bf16(x * rstd); the output is that times the weight, the product left in fp32 for the caller's
+// rounding (norm.cu:72,130-131)
+__device__ __forceinline__ float rms_norm_x(float x, float rstd) {
+  return round_bf16(x * rstd);
+}
+__device__ __forceinline__ uint4 rms_apply_bf16x8(const uint4 x, const uint4 w, float rstd) {
+  const uint32_t* xp = &x.x;
+  const uint32_t* wp = &w.x;
+  uint4 o;
+  uint32_t* op = &o.x;
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float a = rms_norm_x(bf16lo(xp[j]), rstd) * bf16lo(wp[j]);
+    const float b = rms_norm_x(bf16hi(xp[j]), rstd) * bf16hi(wp[j]);
+    op[j] = pack_bf16x2(a, b);
+  }
+  return o;
+}
+
+// rotary pair in bf16 arithmetic, (x, y) -> (rope_x, rope_y): every product and the add / subtract rounded to bf16
+// (rope.cu:52-53)
+__device__ __forceinline__ float rope_x(float x, float y, float c, float s) {
+  return round_bf16(x * c) - round_bf16(y * s);
+}
+__device__ __forceinline__ float rope_y(float x, float y, float c, float s) {
+  return round_bf16(y * c) + round_bf16(x * s);
+}
+// rotated pair (in[xi], in[yi]) -> (out[xi], out[yi]); in place when in == out
+__device__ __forceinline__ void rope_pair(const __nv_bfloat16* in, __nv_bfloat16* out, int xi, int yi, float c, float s) {
+  const float x = __bfloat162float(in[xi]);
+  const float y = __bfloat162float(in[yi]);
+  out[xi] = __float2bfloat16_rn(rope_x(x, y, c, s));
+  out[yi] = __float2bfloat16_rn(rope_y(x, y, c, s));
+}
+__device__ __forceinline__ void rope_pair(__nv_bfloat16* arr, int xi, int yi, float c, float s) {
+  rope_pair(arr, arr, xi, yi, c, s);
+}
+
+// Output side of a qkv projection whose columns are in the rope-pair packed order of quant.pack_w4_qkv_rope (inside every
+// head, packed column 16j+i holds dim 8j+i for i < 8 and dim D/2 + 8j + (i-8) otherwise).
+struct QkvRopeCache {
+  const int64_t* positions;
+  const __nv_bfloat16* cos_sin;   // [max_pos, head_dim] = [cos half | sin half]
+  const int32_t* slots;           // negative: the token is not cached
+  __nv_bfloat16* k_cache;
+  __nv_bfloat16* v_cache;
+  int num_heads, num_kv_heads, head_dim;
+};
+// Packed columns 16 nt + r and 16 nt + r + 8 (r < 8) of token tok, with fp32 values lo / hi: the pair (dims d and
+// d + D/2 of one head), rounded to bf16 as the linear's output, is rotated for q and k heads (rope_x / rope_y, NeoX
+// halves, full rotary), written to row tok of y in logical [q | k | v] column order and, for k / v heads, into the paged
+// caches (reshape_paged_cache.cu:23-62).
+__device__ __forceinline__ void qkv_rope_store(const QkvRopeCache& p, __nv_bfloat16* y, int64_t y_stride, int tok, int nt,
+                                               int r, float lo, float hi) {
+  const int D = p.head_dim, half = D >> 1, tiles_per_head = D >> 4;
+  const int hd = nt / tiles_per_head, d = (nt % tiles_per_head) * 8 + r;
+  float v1 = round_bf16(lo), v2 = round_bf16(hi);
+  const bool is_q = hd < p.num_heads, is_k = !is_q && hd < p.num_heads + p.num_kv_heads;
+  if (is_q || is_k) {
+    const __nv_bfloat16* cs = p.cos_sin + p.positions[tok] * (int64_t)D;
+    const float c = __bfloat162float(cs[d]), sn = __bfloat162float(cs[half + d]);
+    const float o1 = rope_x(v1, v2, c, sn);
+    const float o2 = rope_y(v1, v2, c, sn);
+    v1 = o1;
+    v2 = o2;
+  }
+  const __nv_bfloat16 b1 = __float2bfloat16_rn(v1), b2 = __float2bfloat16_rn(v2);
+  __nv_bfloat16* yr = y + (int64_t)tok * y_stride + (int64_t)hd * D;
+  yr[d] = b1;
+  yr[half + d] = b2;
+  if (!is_q) {
+    const int64_t slot = p.slots[tok];
+    if (slot >= 0) {
+      const int kvh = is_k ? hd - p.num_heads : hd - p.num_heads - p.num_kv_heads;
+      __nv_bfloat16* row = (is_k ? p.k_cache : p.v_cache) + (slot * p.num_kv_heads + kvh) * (int64_t)D;
+      row[d] = b1;
+      row[half + d] = b2;
+    }
+  }
+}
+
+// gate activation in fp32 (activation.cu:97-125); kAct 0 silu, 1 gelu, 2 gelu_tanh.  The bf16 gated form is
+// bf16(act(gate)) * up on bf16 gate and up (activation.cu:35).
+template <int kAct>
+__device__ __forceinline__ float act_fn(float f) {
+  if (kAct == 0) return f / (1.0f + expf(-f));
+  if (kAct == 1) return f * 0.5f * (1.0f + erff(f * 0.70710678118654752440f));
+  const float kBeta = 0.79788456080286535588f;                       // sqrt(2)*2/sqrt(pi)*0.5
+  const float inner = kBeta * (f + 0.044715f * f * f * f);
+  return 0.5f * f * (1.0f + tanhf(inner));
+}
+__device__ __forceinline__ float act_fn(int act_mode, float f) {
+  if (act_mode == 0) return act_fn<0>(f);
+  if (act_mode == 1) return act_fn<1>(f);
+  return act_fn<2>(f);
+}
+
+// SwiGLU on fp32 sums, rounded once by the caller: the MoE experts' form (the fused MoE's fc1 epilogue behind
+// kernels/cuda/moe/fused_moe.cpp:23-124 gates the fp32 accumulators)
+__device__ __forceinline__ float silu_mul_f32(float gate, float up) {
+  return act_fn<0>(gate) * up;
+}
+
 #endif  // __CUDACC__
 }  // namespace xb

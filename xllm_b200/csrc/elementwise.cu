@@ -9,24 +9,6 @@
 namespace xb {
 
 // ---------------------------------------------------------------------------
-// block-wide sum (<=1024 threads)
-// ---------------------------------------------------------------------------
-__device__ __forceinline__ float block_sum(float v, float* smem /*[33]*/) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  v = warp_sum(v);
-  if (lane == 0) smem[warp] = v;
-  __syncthreads();
-  const int nwarps = (blockDim.x + 31) >> 5;
-  if (warp == 0) {
-    float t = lane < nwarps ? smem[lane] : 0.f;
-    t = warp_sum(t);
-    if (lane == 0) smem[32] = t;
-  }
-  __syncthreads();
-  return smem[32];
-}
-
-// ---------------------------------------------------------------------------
 // RMSNorm family.  Reference: xllm/core/kernels/cuda/norm.cu
 //   rms_norm_kernel                         :43-78
 //   fused_add_rms_norm_kernel (width 8)     :80-136
@@ -35,30 +17,6 @@ __device__ __forceinline__ float block_sum(float v, float* smem /*[33]*/) {
 // kVec: 8 bf16 per thread per step, row kept in registers (<= kMaxVec steps),
 // otherwise re-read from L2 (rows > 16K elements).
 // ---------------------------------------------------------------------------
-// ss + sum of squares of the 8 bf16 of x (fp32, in element order)
-__device__ __forceinline__ float sumsq_bf16x8(float ss, const uint4& x) {
-  const uint32_t* xp = &x.x;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    float a = bf16lo(xp[j]), b = bf16hi(xp[j]);
-    ss += a * a + b * b;
-  }
-  return ss;
-}
-// 8 normalised outputs: bf16(x*rstd) then bf16 product with w (norm.cu:75-77,130-133)
-__device__ __forceinline__ uint4 rms_apply_bf16x8(const uint4& x, const uint4& w, float rstd) {
-  const uint32_t* xp = &x.x;
-  const uint32_t* wp = &w.x;
-  uint4 o;
-  uint32_t* op = &o.x;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    float a = round_bf16(bf16lo(xp[j]) * rstd) * bf16lo(wp[j]);
-    float b = round_bf16(bf16hi(xp[j]) * rstd) * bf16hi(wp[j]);
-    op[j] = pack_bf16x2(a, b);
-  }
-  return o;
-}
 
 template <bool kFusedAdd, bool kFp8Out, bool kRoundBeforeFp8>
 __global__ void __launch_bounds__(1024)
@@ -93,12 +51,7 @@ rms_norm_vec_kernel(void* __restrict__ out_, __nv_bfloat16* __restrict__ input,
     if (idx < nvec) {
       uint4 x = in_v[idx];
       if (kFusedAdd) {
-        uint4 r = res_v[idx];
-        uint32_t* xp = &x.x;
-        const uint32_t* rp = &r.x;
-#pragma unroll
-        for (int j = 0; j < 4; ++j)  // bf16 add, one rounding (norm.cu:110-113)
-          xp[j] = pack_bf16x2(bf16lo(xp[j]) + bf16lo(rp[j]), bf16hi(xp[j]) + bf16hi(rp[j]));
+        x = add_bf16x8(x, res_v[idx]);
         res_v[idx] = x;
       }
       ss = sumsq_bf16x8(ss, x);
@@ -109,18 +62,12 @@ rms_norm_vec_kernel(void* __restrict__ out_, __nv_bfloat16* __restrict__ input,
   for (int idx = threadIdx.x + kMaxVec * blockDim.x; idx < nvec; idx += blockDim.x) {
     uint4 x = in_v[idx];
     if (kFusedAdd) {
-      uint4 r = res_v[idx];
-      uint32_t* xp = &x.x;
-      const uint32_t* rp = &r.x;
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        xp[j] = pack_bf16x2(bf16lo(xp[j]) + bf16lo(rp[j]), bf16hi(xp[j]) + bf16hi(rp[j]));
+      x = add_bf16x8(x, res_v[idx]);
       res_v[idx] = x;
     }
     ss = sumsq_bf16x8(ss, x);
   }
-  const float var = block_sum(ss, red);
-  const float rstd = rsqrtf(var / (float)hidden_size + eps);
+  const float rstd = rms_rstd(block_sum(ss, red), hidden_size, eps);
   pdl_launch_dependents();
 
   float inv_scale = 0.f;
@@ -138,8 +85,8 @@ rms_norm_vec_kernel(void* __restrict__ out_, __nv_bfloat16* __restrict__ input,
       uint8_t q[8];
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        float a = round_bf16(bf16lo(xp[j]) * rstd) * bf16lo(wp[j]);
-        float b = round_bf16(bf16hi(xp[j]) * rstd) * bf16hi(wp[j]);
+        float a = rms_norm_x(bf16lo(xp[j]), rstd) * bf16lo(wp[j]);
+        float b = rms_norm_x(bf16hi(xp[j]), rstd) * bf16hi(wp[j]);
         if (kRoundBeforeFp8) {  // width-8 fused path rounds to bf16 first (norm.cu:333-343)
           a = round_bf16(a);
           b = round_bf16(b);
@@ -181,18 +128,17 @@ rms_norm_scalar_kernel(void* __restrict__ out_, __nv_bfloat16* __restrict__ inpu
   for (int i = threadIdx.x; i < hidden_size; i += blockDim.x) {
     float x = __bfloat162float(in[i]);
     if (kFusedAdd) {
-      x = round_bf16(x + __bfloat162float(res[i]));
+      x = add_bf16(x, __bfloat162float(res[i]));
       res[i] = __float2bfloat16_rn(x);
     }
     ss += x * x;
   }
-  const float var = block_sum(ss, red);
-  const float rstd = rsqrtf(var / (float)hidden_size + eps);
+  const float rstd = rms_rstd(block_sum(ss, red), hidden_size, eps);
   pdl_launch_dependents();
   float inv_scale = kFp8Out ? 1.0f / __ldg(fp8_scale) : 0.f;
   for (int i = threadIdx.x; i < hidden_size; i += blockDim.x) {
     float x = __bfloat162float(kFusedAdd ? res[i] : in[i]);
-    float y = round_bf16(x * rstd) * __bfloat162float(weight[i]);
+    float y = rms_norm_x(x, rstd) * __bfloat162float(weight[i]);
     if (kFp8Out) {
       reinterpret_cast<uint8_t*>(out_)[tok * (int64_t)hidden_size + i] = scaled_fp8_e4m3(y, inv_scale);
     } else if (kFusedAdd) {
@@ -294,18 +240,8 @@ __global__ void fp8_scale_finish_kernel(float* scale_out) {
 
 // ---------------------------------------------------------------------------
 // K9 rotary embedding.  rope.cu:27-137: scalar_t arithmetic => every product
-// and the final add/sub are rounded to bf16.
+// and the final add/sub are rounded to bf16 (rope_pair).
 // ---------------------------------------------------------------------------
-// rotated pair (x, y) -> (out[xi], out[yi]); in place when in == out
-__device__ __forceinline__ void rope_pair(const __nv_bfloat16* in, __nv_bfloat16* out, int xi, int yi, float c, float s) {
-  const float x = __bfloat162float(in[xi]);
-  const float y = __bfloat162float(in[yi]);
-  out[xi] = __float2bfloat16_rn(round_bf16(x * c) - round_bf16(y * s));
-  out[yi] = __float2bfloat16_rn(round_bf16(y * c) + round_bf16(x * s));
-}
-__device__ __forceinline__ void rope_pair(__nv_bfloat16* arr, int xi, int yi, float c, float s) {
-  rope_pair(arr, arr, xi, yi, c, s);
-}
 
 template <bool kNeox>
 __global__ void __launch_bounds__(512)
@@ -432,7 +368,7 @@ rope_and_cache_kernel(const int64_t* __restrict__ positions, __nv_bfloat16* __re
 // every head, packed column 16j+i holds dim 8j+i for i < 8 and dim D/2 + 8j + (i-8) otherwise): the decode GEMV
 // applies RoPE + scatter in its own epilogue; this kernel serves the same weights when the projection ran as a plain
 // GEMM (prefill, decode batches > 8).  Reads the packed row, writes q / k / v in LOGICAL order to qkv_out and the new
-// k / v rows into the paged caches.  Same arithmetic as rope_pair (rope.cu:27-54), NeoX halves, full rotary.
+// k / v rows into the paged caches, with the GEMV epilogue's qkv_rope_store.
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(512)
 rope_and_cache_packed_kernel(const int64_t* __restrict__ positions, const __nv_bfloat16* __restrict__ qkv_packed,
@@ -443,34 +379,13 @@ rope_and_cache_packed_kernel(const int64_t* __restrict__ positions, const __nv_b
   const int64_t tok = blockIdx.x;
   pdl_launch_dependents();
   pdl_wait();
-  const int64_t pos = positions[tok];
-  const int64_t slot = slot_ids[tok];
-  const int half = head_size >> 1;
-  const __nv_bfloat16* cache = cos_sin_cache + pos * head_size;
+  const QkvRopeCache p{positions, cos_sin_cache, slot_ids, key_cache, value_cache, num_heads, num_kv_heads, head_size};
   const __nv_bfloat16* in = qkv_packed + tok * in_stride;
-  __nv_bfloat16* out = qkv_out + tok * out_stride;
-  const int total_heads = num_heads + 2 * num_kv_heads;
-  for (int i = threadIdx.x; i < total_heads * half; i += blockDim.x) {
-    const int hd = i / half, r = i % half;
-    const int p1 = hd * head_size + 16 * (r >> 3) + (r & 7);
-    float v1 = __bfloat162float(in[p1]), v2 = __bfloat162float(in[p1 + 8]);
-    const bool is_q = hd < num_heads, is_k = !is_q && hd < num_heads + num_kv_heads;
-    if (is_q || is_k) {
-      const float c = __bfloat162float(cache[r]), sn = __bfloat162float(cache[half + r]);
-      const float o1 = round_bf16(v1 * c) - round_bf16(v2 * sn);
-      const float o2 = round_bf16(v2 * c) + round_bf16(v1 * sn);
-      v1 = o1;
-      v2 = o2;
-    }
-    const __nv_bfloat16 b1 = __float2bfloat16_rn(v1), b2 = __float2bfloat16_rn(v2);
-    out[hd * head_size + r] = b1;
-    out[hd * head_size + half + r] = b2;
-    if (!is_q && slot >= 0) {
-      const int kvh = is_k ? hd - num_heads : hd - num_heads - num_kv_heads;
-      __nv_bfloat16* row = (is_k ? key_cache : value_cache) + (slot * num_kv_heads + kvh) * (int64_t)head_size;
-      row[r] = b1;
-      row[half + r] = b2;
-    }
+  const int pairs = (num_heads + 2 * num_kv_heads) * (head_size >> 1);
+  for (int i = threadIdx.x; i < pairs; i += blockDim.x) {
+    const int nt = i >> 3, r = i & 7;   // packed columns 16 nt + r and 16 nt + r + 8
+    qkv_rope_store(p, qkv_out, out_stride, (int)tok, nt, r, __bfloat162float(in[16 * nt + r]),
+                   __bfloat162float(in[16 * nt + r + 8]));
   }
   pdl_launch_dependents();
 }
@@ -551,14 +466,6 @@ fused_qk_norm_rope_kernel(__nv_bfloat16* __restrict__ qkv, int num_heads_q, int 
 // K11 act_and_mul.  activation.cu:45-130: act in fp32, rounded to bf16, then a
 // bf16 multiply (second rounding).
 // ---------------------------------------------------------------------------
-template <int kAct>
-__device__ __forceinline__ float act_fn(float f) {
-  if (kAct == 0) return f / (1.0f + expf(-f));                       // silu_kernel :97-102
-  if (kAct == 1) return f * 0.5f * (1.0f + erff(f * 0.70710678118654752440f));  // gelu :104-112
-  const float kBeta = 0.79788456080286535588f;                       // sqrt(2)*2/sqrt(pi)*0.5
-  const float inner = kBeta * (f + 0.044715f * f * f * f);           // gelu_tanh :114-125
-  return 0.5f * f * (1.0f + tanhf(inner));
-}
 
 template <int kAct>
 __global__ void __launch_bounds__(1024)
@@ -643,8 +550,7 @@ mla_cache_latent_kernel(const __nv_bfloat16* __restrict__ latent, int64_t latent
   if (slot < 0) return;  // uniform over the CTA
   const __nv_bfloat16* row = latent + tok * latent_stride;
   const uint4 x = reinterpret_cast<const uint4*>(row)[threadIdx.x];
-  const float var = block_sum(sumsq_bf16x8(0.f, x), red);
-  const float rstd = rsqrtf(var / (float)kDc + eps);
+  const float rstd = rms_rstd(block_sum(sumsq_bf16x8(0.f, x), red), kDc, eps);
   const int64_t page = slot / page_size, off = slot % page_size;
   reinterpret_cast<uint4*>(ckv_cache + page * ckv_stride_page + off * ckv_stride_token)[threadIdx.x] =
       rms_apply_bf16x8(x, w, rstd);

@@ -370,7 +370,7 @@ gemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_const
 #pragma unroll
               for (int e = 0; e < 2; ++e) {
                 const float up = acc[4 * j + 2 * h + e], gate = acc[4 * (j + Cfg::kAcc / 8) + 2 * h + e];
-                o[e] = (gate / (1.0f + expf(-gate))) * up;     // silu(gate) * up on the fp32 sums, as the GEMV path
+                o[e] = silu_mul_f32(gate, up);
               }
               *reinterpret_cast<uint32_t*>(crow + col) = pack_bf16x2(o[0], o[1]);
             }

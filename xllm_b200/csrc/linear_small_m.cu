@@ -92,15 +92,10 @@ struct W4Fuse {
   // split RMSNorm: the PRODUCER linear (epilogue 3: o_proj / down_proj) adds the residual, writes the updated residual
   // stream r = bf16(bf16(y) + residual) to res_out and the per-(16-row tile, token) sums of r^2 to stats_out
   // [N/16][8]; the CONSUMER linear (stats_in != null: qkv / gate_up) reads r as its x, sums the K/16 partials in a
-  // fixed order and normalises while staging x in shared memory - one L2 round trip, no reduction over K in any CTA.
+  // fixed order and normalises x once it is staged in shared memory - no reduction over K in any CTA.
   const float* stats_in;
   float* stats_out;
-  const int64_t* positions;
-  const __nv_bfloat16* cos_sin;   // [max_pos, head_dim] = [cos half | sin half]
-  const int32_t* slots;
-  __nv_bfloat16* k_cache;
-  __nv_bfloat16* v_cache;
-  int num_heads, num_kv_heads, head_dim;
+  QkvRopeCache rope;   // epilogue 2
 };
 
 template <int kMT /* n8 token tiles: M <= 8*kMT */, int kSplit /* 1,2,4,8 warps per row tile */, int kDepth,
@@ -190,46 +185,8 @@ linear_w4a16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, con
   if constexpr (kXs) {
     const int nvec = K >> 3;
     const bool do_norm = fz.norm_w != nullptr;
-    if (fz.stats_in != nullptr) {
-      // ---- consumer of a split RMSNorm: x IS the residual stream; sum(x^2) per token arrives as K/16 partials ----
-      // every load (x vectors, partials, norm weights) is issued up front: one round trip to L2
-      const int nst = K >> 4;
-      float part[8];
-#pragma unroll
-      for (int tk = 0; tk < 8; ++tk) part[tk] = 0.f;
-      for (int i = threadIdx.x; i < nst; i += kWarps * 32) {      // fixed assignment -> every CTA gets the same bits
-        const float4 a = __ldcg(reinterpret_cast<const float4*>(fz.stats_in + (int64_t)i * 8));
-        const float4 b = __ldcg(reinterpret_cast<const float4*>(fz.stats_in + (int64_t)i * 8 + 4));
-        part[0] += a.x; part[1] += a.y; part[2] += a.z; part[3] += a.w;
-        part[4] += b.x; part[5] += b.y; part[6] += b.z; part[7] += b.w;
-      }
-#pragma unroll
-      for (int tk = 0; tk < 8; ++tk) {
-        const float v = warp_sum(part[tk]);
-        if (lane == 0) s_ss[warp][tk] = v;
-      }
-      __syncthreads();
-      const uint4* wv = reinterpret_cast<const uint4*>(fz.norm_w);
-      for (int tok = 0; tok < M; ++tok) {
-        float var = 0.f;
-#pragma unroll
-        for (int w = 0; w < kWarps; ++w) var += s_ss[w][tok];
-        const float rstd = rsqrtf(var / (float)K + fz.eps);
-        const uint4* src = reinterpret_cast<const uint4*>(x + (int64_t)tok * x_stride);
-        uint4* dst = reinterpret_cast<uint4*>(xs + (int64_t)tok * xs_stride);
-        for (int idx = threadIdx.x; idx < nvec; idx += kWarps * 32) {
-          uint4 v = src[idx];
-          const uint4 w = __ldg(wv + idx);
-          uint32_t* vp = &v.x;
-          const uint32_t* wq = &w.x;
-#pragma unroll
-          for (int j = 0; j < 4; ++j)  // bf16(x*rstd) then bf16 product with w (norm.cu:75-77,130-133)
-            vp[j] = pack_bf16x2(round_bf16(bf16lo(vp[j]) * rstd) * bf16lo(wq[j]), round_bf16(bf16hi(vp[j]) * rstd) * bf16hi(wq[j]));
-          dst[idx] = v;
-        }
-      }
-      __syncthreads();
-    } else {
+    // split RMSNorm consumer: x IS the residual stream and sum(x^2) per token arrives as K/16 partials
+    const bool split_norm = fz.stats_in != nullptr;
     for (int tok = 0; tok < M; ++tok) {
       const uint4* src = reinterpret_cast<const uint4*>(x + (int64_t)tok * x_stride);
       // (under epilogue 3 the residual pointers belong to the EPILOGUE - the [M, N] residual stream - not to x)
@@ -258,51 +215,46 @@ linear_w4a16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, con
       }
       for (int idx = threadIdx.x; idx < nvec; idx += kWarps * 32) {
         uint4 v = src[idx];
-        if (rsrc) {
-          const uint4 r = rsrc[idx];
-          uint32_t* vp = &v.x;
-          const uint32_t* rp = &r.x;
-#pragma unroll
-          for (int j = 0; j < 4; ++j)  // bf16 add, one rounding (norm.cu:110-113)
-            vp[j] = pack_bf16x2(bf16lo(vp[j]) + bf16lo(rp[j]), bf16hi(vp[j]) + bf16hi(rp[j]));
-        }
+        if (rsrc) v = add_bf16x8(v, rsrc[idx]);
         if (rdst) rdst[idx] = v;
-        const uint32_t* vp = &v.x;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          const float a = bf16lo(vp[j]), b = bf16hi(vp[j]);
-          ss += a * a + b * b;
-        }
+        ss = sumsq_bf16x8(ss, v);
         dst[idx] = v;
       }
-      if (do_norm) {
+      if (do_norm && !split_norm) {
         ss = warp_sum(ss);
         if (lane == 0) s_ss[warp][tok] = ss;
       }
     }
+    if (split_norm) {
+      float part[8];
+#pragma unroll
+      for (int tk = 0; tk < 8; ++tk) part[tk] = 0.f;
+      for (int i = threadIdx.x; i < (K >> 4); i += kWarps * 32) {      // fixed assignment -> every CTA gets the same bits
+        const float4 a = __ldcg(reinterpret_cast<const float4*>(fz.stats_in + (int64_t)i * 8));
+        const float4 b = __ldcg(reinterpret_cast<const float4*>(fz.stats_in + (int64_t)i * 8 + 4));
+        part[0] += a.x; part[1] += a.y; part[2] += a.z; part[3] += a.w;
+        part[4] += b.x; part[5] += b.y; part[6] += b.z; part[7] += b.w;
+      }
+#pragma unroll
+      for (int tk = 0; tk < 8; ++tk) {
+        const float v = warp_sum(part[tk]);
+        if (lane == 0) s_ss[warp][tk] = v;
+      }
+    }
     if (do_norm) {
       __syncthreads();
+      const uint4* wv = reinterpret_cast<const uint4*>(fz.norm_w);
       for (int tok = 0; tok < M; ++tok) {
         float var = 0.f;
 #pragma unroll
         for (int w = 0; w < kWarps; ++w) var += s_ss[w][tok];       // fixed order: every CTA gets the same rstd
-        const float rstd = rsqrtf(var / (float)K + fz.eps);
+        const float rstd = rms_rstd(var, K, fz.eps);
         uint4* dst = reinterpret_cast<uint4*>(xs + (int64_t)tok * xs_stride);
-        const uint4* wv = reinterpret_cast<const uint4*>(fz.norm_w);
-        for (int idx = threadIdx.x; idx < nvec; idx += kWarps * 32) {   // same elements this thread wrote above
-          uint4 v = dst[idx];
-          const uint4 w = __ldg(wv + idx);
-          uint32_t* vp = &v.x;
-          const uint32_t* wq = &w.x;
-#pragma unroll
-          for (int j = 0; j < 4; ++j)  // bf16(x*rstd) then bf16 product with w (norm.cu:75-77,130-133)
-            vp[j] = pack_bf16x2(round_bf16(bf16lo(vp[j]) * rstd) * bf16lo(wq[j]), round_bf16(bf16hi(vp[j]) * rstd) * bf16hi(wq[j]));
-          dst[idx] = v;
-        }
+        for (int idx = threadIdx.x; idx < nvec; idx += kWarps * 32)   // same elements this thread staged above
+          dst[idx] = rms_apply_bf16x8(dst[idx], __ldg(wv + idx), rstd);
       }
     }
     __syncthreads();
-    }
   }
 
   // x fragments: lane (g,t) needs x[tok = 8m+g][k0 + 16t .. +16) per tile
@@ -449,41 +401,7 @@ linear_w4a16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, con
   // N/2 values per token are written - the separate act_and_mul launch and its 3*N bytes of traffic disappear.
   auto gate_up = [&](float gate, float up) -> __nv_bfloat16 {
     const float gr = round_bf16(gate), ur = round_bf16(up);
-    float a;
-    if (act_mode == 0) a = gr / (1.0f + expf(-gr));
-    else if (act_mode == 1) a = gr * 0.5f * (1.0f + erff(gr * 0.70710678118654752440f));
-    else a = 0.5f * gr * (1.0f + tanhf(0.79788456080286535588f * (gr + 0.044715f * gr * gr * gr)));
-    return __float2bfloat16_rn(round_bf16(a) * ur);
-  };
-  // kEpi == 2: (lo, hi) are the fp32 sums (+bias) of dims d and d + head_dim/2 of head `hd` for token `tok`: round to
-  // bf16 (the linear's output), rotate q / k heads (rope.cu:27-54: every product and the add / sub rounded to bf16),
-  // write q (and k, v) to y in LOGICAL column order and the new token's k / v rows into the paged caches.
-  auto rope_store = [&](int nt, int r, int tok, float lo, float hi) {
-    const int D = fz.head_dim, half = D >> 1, tiles_per_head = D >> 4;
-    const int hd = nt / tiles_per_head, d = (nt % tiles_per_head) * 8 + r;
-    float v1 = round_bf16(lo), v2 = round_bf16(hi);
-    const bool is_q = hd < fz.num_heads, is_k = !is_q && hd < fz.num_heads + fz.num_kv_heads;
-    if (is_q || is_k) {
-      const __nv_bfloat16* cs = fz.cos_sin + fz.positions[tok] * (int64_t)D;
-      const float c = __bfloat162float(cs[d]), sn = __bfloat162float(cs[half + d]);
-      const float o1 = round_bf16(v1 * c) - round_bf16(v2 * sn);
-      const float o2 = round_bf16(v2 * c) + round_bf16(v1 * sn);
-      v1 = o1;
-      v2 = o2;
-    }
-    const __nv_bfloat16 b1 = __float2bfloat16_rn(v1), b2 = __float2bfloat16_rn(v2);
-    __nv_bfloat16* yr = y + (int64_t)tok * y_stride + (int64_t)hd * D;
-    yr[d] = b1;
-    yr[half + d] = b2;
-    if (!is_q) {
-      const int64_t slot = fz.slots[tok];
-      if (slot >= 0) {
-        const int kvh = is_k ? hd - fz.num_heads : hd - fz.num_heads - fz.num_kv_heads;
-        __nv_bfloat16* row = (is_k ? fz.k_cache : fz.v_cache) + (slot * fz.num_kv_heads + kvh) * (int64_t)D;
-        row[d] = b1;
-        row[half + d] = b2;
-      }
-    }
+    return __float2bfloat16_rn(round_bf16(act_fn(act_mode, gr)) * ur);
   };
   if constexpr (kSplit == 1) {
     if (live) {
@@ -497,7 +415,7 @@ linear_w4a16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, con
               float gv = acc[m][e], uv = acc[m][2 + e];
               if (bias) { gv += __bfloat162float(bias[n0 + g]); uv += __bfloat162float(bias[n0 + g + 8]); }
               if constexpr (kGateUp) y[(int64_t)tok * y_stride + ntile * 8 + g] = gate_up(gv, uv);
-              else rope_store(ntile, g, tok, gv, uv);
+              else qkv_rope_store(fz.rope, y, y_stride, tok, ntile, g, gv, uv);
             }
           }
         } else {
@@ -535,12 +453,12 @@ linear_w4a16_small_m_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, con
             for (int w = 0; w < kSplit; ++w) up += red[tl * kSplit + w][m][(r + 8) * 8 + c];
             if (bias) up += __bfloat162float(bias[nt * 16 + r + 8]);
             if constexpr (kGateUp) y[(int64_t)tok * y_stride + nt * 8 + r] = gate_up(sum, up);
-            else rope_store(nt, r, tok, sum, up);
+            else qkv_rope_store(fz.rope, y, y_stride, tok, nt, r, sum, up);
           }
         } else if constexpr (kEpi == 3) {
           // producer half of the split RMSNorm (fused_add_rms_norm, norm.cu:80-136): r = bf16(bf16(y) + residual)
           const int n = nt * 16 + r;
-          const float rr = round_bf16(round_bf16(sum) + __bfloat162float(fz.res_in[(int64_t)tok * N + n]));
+          const float rr = add_bf16(round_bf16(sum), __bfloat162float(fz.res_in[(int64_t)tok * N + n]));
           fz.res_out[(int64_t)tok * N + n] = __float2bfloat16_rn(rr);
           s_sq[tl][r][c] = rr * rr;
         } else {
@@ -895,14 +813,9 @@ extern "C" int xb_linear_w4a16_decode_fused(void* y, int64_t y_stride, const voi
     XB_CHECK((head_dim == 64 || head_dim == 128) && num_heads > 0 && num_kv_heads > 0 &&
                  N == (num_heads + 2 * num_kv_heads) * head_dim,
              "linear_w4a16_decode_fused: N=%d is not (%d + 2*%d) heads of %d", N, num_heads, num_kv_heads, head_dim);
-    fz.positions = positions;
-    fz.cos_sin = reinterpret_cast<const __nv_bfloat16*>(cos_sin_cache);
-    fz.slots = slot_ids;
-    fz.k_cache = reinterpret_cast<__nv_bfloat16*>(k_cache);
-    fz.v_cache = reinterpret_cast<__nv_bfloat16*>(v_cache);
-    fz.num_heads = num_heads;
-    fz.num_kv_heads = num_kv_heads;
-    fz.head_dim = head_dim;
+    fz.rope = QkvRopeCache{positions, reinterpret_cast<const __nv_bfloat16*>(cos_sin_cache), slot_ids,
+                           reinterpret_cast<__nv_bfloat16*>(k_cache), reinterpret_cast<__nv_bfloat16*>(v_cache),
+                           num_heads, num_kv_heads, head_dim};
   }
   const bool xs = norm_weight != nullptr || stage_x != 0;
   return w4_small_m_impl(y, y_stride, x, x_stride, qweight, meta, bias, M, N, K, group_size, epilogue, act_mode, xs, &fz, stream);

@@ -215,7 +215,7 @@ moe_expert_gemv_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, const __
         if (kSwiGLU) s1 += red[ww][1][r];
       }
       float out = s0;
-      if (kSwiGLU) out = (s1 / (1.0f + expf(-s1))) * s0;      // silu(gate) * up on the fp32 sums
+      if (kSwiGLU) out = silu_mul_f32(s1, s0);
       y[(int64_t)pair * y_stride + n0 + r] = __float2bfloat16_rn(mine ? out : 0.f);
     }
   }
@@ -322,7 +322,7 @@ moe_expert_gemv_w4_kernel(__nv_bfloat16* __restrict__ y, int64_t y_stride, const
         if (kSwiGLU) s1 += red[ww][1][r];
       }
       float out = s0;
-      if (kSwiGLU) out = (s1 / (1.0f + expf(-s1))) * s0;
+      if (kSwiGLU) out = silu_mul_f32(s1, s0);
       y[(int64_t)pair * y_stride + n0 + r] = __float2bfloat16_rn(mine ? out : 0.f);
     }
   }
