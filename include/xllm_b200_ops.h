@@ -479,6 +479,8 @@ int xb_set_fp8_splitk_max(int max_split);   /* 1 = never split .. 32; default 8 
  * peer_data[r] / peer_flags[r]: device pointers, valid on THIS GPU, to rank r's symmetric partial buffer and signal
  * pad ([max_ctas][8] uint32, zero-initialised once); epoch: local uint32[max_ctas], zero-initialised once.
  * Sum order is rank 0..world-1 in fp32, one rounding: bit-identical on all ranks.
+ * out / residual / weight / peer_data[r] must be 16-byte aligned, peer_flags[r] / epoch 4-byte aligned; numel >= 0,
+ * max_ctas >= 1, 0 < hidden <= 16384, 0 <= num_tokens <= max_ctas.  Anything else is refused before any launch.
  * xb_allreduce_add_rms_norm_bf16 fuses the exchange with the fused_add_rms_norm that follows every row-parallel
  * linear: residual <- bf16(allreduce(partials)) + residual; out <- rms_norm(residual) * weight. */
 int xb_oneshot_allreduce_bf16(void* out, const void* const* peer_data, void* const* peer_flags,

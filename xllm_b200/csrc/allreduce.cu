@@ -132,7 +132,8 @@ allreduce_add_rms_norm_kernel(__nv_bfloat16* __restrict__ out, __nv_bfloat16* __
     }
   }
   // the residual add, squares and block sum above are add_bf16x8 / sumsq_bf16x8 / block_sum written out on the fp32
-  // all-reduce sums: through the helpers this kernel, which no single-GPU test runs, compiles to different code
+  // all-reduce sums (through the helpers this kernel compiles to different code); tests/test_gpu_peer_exchange.py holds
+  // it bit-identical to oneshot_allreduce followed by fused_add_rms_norm
   ss = warp_sum(ss);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = ss;
   __syncthreads();
@@ -157,8 +158,16 @@ allreduce_add_rms_norm_kernel(__nv_bfloat16* __restrict__ out, __nv_bfloat16* __
 
 using namespace xb;
 
+static inline bool aligned(const void* p, uintptr_t bytes) { return (reinterpret_cast<uintptr_t>(p) & (bytes - 1)) == 0; }
+
+// The kernels move data as uint4 and signals / epochs as uint32: a misaligned pointer would fault the GPU, so it is refused.
 static int fill_peers(PeerPtrs& pp, const void* const* peer_data, void* const* peer_flags, void* epoch, int rank, int world) {
   XB_CHECK(world >= 1 && world <= kMaxRanks && rank >= 0 && rank < world, "allreduce: bad rank %d / world %d", rank, world);
+  for (int r = 0; r < world; ++r) {
+    XB_CHECK(aligned(peer_data[r], 16), "allreduce: peer_data[%d] %p is not 16-byte aligned", r, peer_data[r]);
+    XB_CHECK(aligned(peer_flags[r], 4), "allreduce: peer_flags[%d] %p is not 4-byte aligned", r, peer_flags[r]);
+  }
+  XB_CHECK(aligned(epoch, 4), "allreduce: epoch %p is not 4-byte aligned", epoch);
   for (int r = 0; r < kMaxRanks; ++r) {
     pp.data[r] = r < world ? reinterpret_cast<const __nv_bfloat16*>(peer_data[r]) : nullptr;
     pp.flags[r] = r < world ? reinterpret_cast<uint32_t*>(peer_flags[r]) : nullptr;
@@ -173,12 +182,14 @@ extern "C" int xb_oneshot_allreduce_bf16(void* out, const void* const* peer_data
                                          int rank, int world, int64_t numel, int max_ctas, xb_stream_t stream) {
   if (numel == 0) return 0;
   XB_CHECK(numel % 8 == 0, "oneshot_allreduce: numel %lld must be a multiple of 8", (long long)numel);
+  XB_CHECK(numel > 0, "oneshot_allreduce: numel %lld must not be negative", (long long)numel);
+  XB_CHECK(max_ctas >= 1, "oneshot_allreduce: max_ctas %d must be at least 1", max_ctas);
   PeerPtrs pp;
   if (fill_peers(pp, peer_data, peer_flags, epoch, rank, world)) return 1;
+  XB_CHECK(aligned(out, 16), "oneshot_allreduce: out %p is not 16-byte aligned", out);
   int64_t n_vec = numel / 8;
   int ctas = (int)((n_vec + 511) / 512);
   if (ctas > max_ctas) ctas = max_ctas;
-  if (ctas < 1) ctas = 1;
   XB_CUDA_OK(launch(oneshot_allreduce_kernel, dim3(ctas), dim3(512), 0, (cudaStream_t)stream, true,
                     reinterpret_cast<__nv_bfloat16*>(out), pp, n_vec));
   return 0;
@@ -188,11 +199,15 @@ extern "C" int xb_allreduce_add_rms_norm_bf16(void* out, void* residual, const v
                                               void* const* peer_flags, void* epoch, int rank, int world, float eps,
                                               int num_tokens, int hidden, int max_ctas, xb_stream_t stream) {
   if (num_tokens == 0) return 0;
-  XB_CHECK(hidden % 8 == 0 && hidden <= 16384, "allreduce_add_rms_norm: hidden %d must be a multiple of 8 and <= 16384", hidden);
+  XB_CHECK(hidden > 0 && hidden % 8 == 0 && hidden <= 16384,
+           "allreduce_add_rms_norm: hidden %d must be a positive multiple of 8 and <= 16384", hidden);
   XB_CHECK(num_tokens <= max_ctas, "allreduce_add_rms_norm: %d tokens exceed the %d flag slots (use NCCL for prefill-sized messages)",
            num_tokens, max_ctas);
+  XB_CHECK(num_tokens > 0, "allreduce_add_rms_norm: num_tokens %d must not be negative", num_tokens);
   PeerPtrs pp;
   if (fill_peers(pp, peer_data, peer_flags, epoch, rank, world)) return 1;
+  XB_CHECK(aligned(out, 16) && aligned(residual, 16) && aligned(weight, 16),
+           "allreduce_add_rms_norm: out %p / residual %p / weight %p must be 16-byte aligned", out, residual, weight);
   int threads = ((hidden / 8 + 31) / 32) * 32;
   if (threads > 1024) threads = 1024;
   XB_CUDA_OK(launch(allreduce_add_rms_norm_kernel, dim3(num_tokens), dim3(threads), 0, (cudaStream_t)stream, true,
