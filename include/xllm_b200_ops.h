@@ -144,6 +144,23 @@ int xb_fused_qk_norm_rope_bf16(void* qkv, int num_heads_q, int num_heads_k,
                                int interleaved, const int64_t* position_ids,
                                int num_tokens, xb_stream_t stream);
 
+/* ---- K10+K12 fused: QK-norm + RoPE (q,k in place) + scatter of k and v -----
+ * one launch instead of fused_qk_norm_rope + reshape_paged_cache
+ * (qwen2_attention.cpp:147-171 + flashinfer_attention.cpp:128-131).
+ * qkv contiguous [T,(hq+2*hkv)*d], d = 64 or 128; NeoX halves, full rotary
+ * (cos_sin_cache [max_pos, d]); caches NHD [n_blocks, block_size, hkv, d];
+ * slot<0 skips the cache writes only.  qkv and both caches are bit-identical
+ * to calling the two ops in sequence.  Other head_dim and NULL weights or
+ * table are rejected before any device access; num_tokens == 0 is a no-op. */
+int xb_qk_norm_rope_and_cache_bf16(void* qkv, int num_heads_q, int num_heads_kv,
+                                   int head_dim, float eps, const void* q_weight,
+                                   const void* k_weight,
+                                   const void* cos_sin_cache,
+                                   const int64_t* positions,
+                                   const int32_t* slot_ids, void* key_cache,
+                                   void* value_cache, int num_tokens,
+                                   xb_stream_t stream);
+
 /* ---- K11: act_and_mul ------------------------------------------------------
  * replaces xllm::kernel::cuda::act_and_mul (cuda_ops_api.h:39-42,
  * activation.cu:45-186).  out[t,:] = bf16( bf16(act(x[t,:d])) * x[t,d:] ).

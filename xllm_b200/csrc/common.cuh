@@ -368,6 +368,49 @@ __device__ __forceinline__ void rope_pair(__nv_bfloat16* arr, int xi, int yi, fl
   rope_pair(arr, arr, xi, yi, c, s);
 }
 
+// Qwen3 per-head RMSNorm + RoPE on one warp (fused_qknorm_rope.cu:84-300): lane owns the kHeadDim / 32 consecutive
+// elements e of one head and the matching weights w.  Norm in fp32 (e *= rstd * w, :197-202), rotation in fp32 over the
+// first rot_dim elements of the [cos | sin] row `cache`, no rounding: the caller rounds once at the store.
+template <int kHeadDim, bool kInterleave>
+__device__ __forceinline__ void qk_norm_rope_warp(float (&e)[kHeadDim / 32], const float (&w)[kHeadDim / 32], float eps,
+                                                  const __nv_bfloat16* cache, int rot_dim, int lane) {
+  constexpr int kPerLane = kHeadDim / 32;
+  float ss = 0.f;
+#pragma unroll
+  for (int i = 0; i < kPerLane; ++i) ss += e[i] * e[i];
+  ss = warp_sum(ss);
+  const float rstd = rsqrtf(ss / (float)kHeadDim + eps);
+#pragma unroll
+  for (int i = 0; i < kPerLane; ++i) e[i] *= rstd * w[i];
+  const int embed = rot_dim / 2;
+  if (kInterleave) {
+    // pairs (2r, 2r+1) are both inside the lane (kPerLane even)
+#pragma unroll
+    for (int i = 0; i < kPerLane; i += 2) {
+      const int d = lane * kPerLane + i;
+      if (d < rot_dim) {
+        const float c = __bfloat162float(cache[d / 2]), s = __bfloat162float(cache[embed + d / 2]);
+        const float x = e[i], y = e[i + 1];
+        e[i] = x * c - y * s;
+        e[i + 1] = y * c + x * s;
+      }
+    }
+  } else {
+    // NeoX: pair (r, r+embed); partner lives in lane ^ (embed / kPerLane) when rot_dim == head_dim
+    const int lanes_half = embed / kPerLane;
+#pragma unroll
+    for (int i = 0; i < kPerLane; ++i) {
+      const int d = lane * kPerLane + i;
+      const float partner = __shfl_xor_sync(0xffffffffu, e[i], lanes_half);
+      if (d < rot_dim) {
+        const int r = d < embed ? d : d - embed;
+        const float c = __bfloat162float(cache[r]), s = __bfloat162float(cache[embed + r]);
+        e[i] = d < embed ? e[i] * c - partner * s : e[i] * c + partner * s;
+      }
+    }
+  }
+}
+
 // Output side of a qkv projection whose columns are in the rope-pair packed order of quant.pack_w4_qkv_rope (inside every
 // head, packed column 16j+i holds dim 8j+i for i < 8 and dim D/2 + 8j + (i-8) otherwise).
 struct QkvRopeCache {

@@ -1,9 +1,11 @@
 // HBM-bound elementwise ops between the linears and attention:
 //   K7/K8 RMSNorm(+residual)(+static FP8 quant), K6 FP8 quant, K9 RoPE,
-//   K12 KV scatter, K9+K12 fused, K10 QK-norm+RoPE, K11 act_and_mul.
+//   K12 KV scatter, K9+K12 fused, K10 QK-norm+RoPE, K10+K12 fused, K11 act_and_mul.
 // Rounding order follows the reference kernels exactly (see each kernel).
 // All kernels: 16-byte vectorised accesses, one CTA (or a few warps) per token,
 // PDL-aware (griddepcontrol) so they chain inside a CUDA graph without bubbles.
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace xb {
@@ -415,50 +417,73 @@ fused_qk_norm_rope_kernel(__nv_bfloat16* __restrict__ qkv, int num_heads_q, int 
   const int total_heads = num_heads_q + num_heads_k + num_heads_v;
   __nv_bfloat16* ptr = qkv + ((int64_t)tok * total_heads + head) * kHeadDim;
   const __nv_bfloat16* w = is_q ? q_weight : k_weight;
-  float e[kPerLane];
-  float ss = 0.f;
+  float e[kPerLane], wf[kPerLane];
   // lane owns kPerLane consecutive elements
 #pragma unroll
   for (int i = 0; i < kPerLane; ++i) {
     e[i] = __bfloat162float(ptr[lane * kPerLane + i]);
-    ss += e[i] * e[i];
+    wf[i] = __bfloat162float(w[lane * kPerLane + i]);
   }
-  ss = warp_sum(ss);
-  const float rstd = rsqrtf(ss / (float)kHeadDim + eps);
-#pragma unroll
-  for (int i = 0; i < kPerLane; ++i) e[i] *= rstd * __bfloat162float(w[lane * kPerLane + i]);  // :197-202
-
-  const int64_t pos = position_ids[tok];
-  const __nv_bfloat16* cache = cos_sin_cache + pos * rot_dim;
-  const int embed = rot_dim / 2;
-  if (kInterleave) {
-    // pairs (2r, 2r+1) are both inside the lane (kPerLane even)
-#pragma unroll
-    for (int i = 0; i < kPerLane; i += 2) {
-      const int d = lane * kPerLane + i;
-      if (d < rot_dim) {
-        const float c = __bfloat162float(cache[d / 2]), s = __bfloat162float(cache[embed + d / 2]);
-        const float x = e[i], y = e[i + 1];
-        e[i] = x * c - y * s;
-        e[i + 1] = y * c + x * s;
-      }
-    }
-  } else {
-    // NeoX: pair (r, r+embed); partner lives in lane ^ (embed / kPerLane) when rot_dim == head_dim
-    const int lanes_half = embed / kPerLane;
-#pragma unroll
-    for (int i = 0; i < kPerLane; ++i) {
-      const int d = lane * kPerLane + i;
-      const float partner = __shfl_xor_sync(0xffffffffu, e[i], lanes_half);
-      if (d < rot_dim) {
-        const int r = d < embed ? d : d - embed;
-        const float c = __bfloat162float(cache[r]), s = __bfloat162float(cache[embed + r]);
-        e[i] = d < embed ? e[i] * c - partner * s : e[i] * c + partner * s;
-      }
-    }
-  }
+  qk_norm_rope_warp<kHeadDim, kInterleave>(e, wf, eps, cos_sin_cache + position_ids[tok] * rot_dim, rot_dim, lane);
 #pragma unroll
   for (int i = 0; i < kPerLane; ++i) ptr[lane * kPerLane + i] = __float2bfloat16_rn(e[i]);
+  pdl_launch_dependents();
+}
+
+// ---------------------------------------------------------------------------
+// K10+K12 fused (Qwen3): per-head RMSNorm + NeoX RoPE of q and k in place, then the normalised, rotated k row and the
+// untouched v row into the NHD paged caches (slot < 0: no cache write).  One warp per (token, head) over
+// Hq + 2 Hkv heads; v-head warps only copy.  Norm + RoPE are qk_norm_rope_warp and the store rounds once, as
+// fused_qk_norm_rope_kernel does, so qkv and both caches are bit-identical to K10 followed by K12.
+// ---------------------------------------------------------------------------
+template <int kHeadDim>
+__global__ void __launch_bounds__(256)
+qk_norm_rope_and_cache_kernel(__nv_bfloat16* __restrict__ qkv, int num_heads_q, int num_heads_kv, float eps,
+                              const __nv_bfloat16* __restrict__ q_weight, const __nv_bfloat16* __restrict__ k_weight,
+                              const __nv_bfloat16* __restrict__ cos_sin_cache, const int64_t* __restrict__ positions,
+                              const int32_t* __restrict__ slot_ids, __nv_bfloat16* __restrict__ key_cache,
+                              __nv_bfloat16* __restrict__ value_cache, int num_tokens) {
+  constexpr int kPerLane = kHeadDim / 32;   // 2 or 4 bf16: one 4- or 8-byte access per lane
+  using Vec = typename std::conditional<kPerLane == 4, uint2, uint32_t>::type;
+  const int warp_global = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  const int heads = num_heads_q + 2 * num_heads_kv;
+  const int tok = warp_global / heads;
+  const int head = warp_global % heads;
+  if (tok >= num_tokens) return;
+  const bool is_q = head < num_heads_q, is_v = head >= num_heads_q + num_heads_kv;
+  // norm weights do not depend on the producer kernel: fetch before the PDL wait
+  float w[kPerLane];
+  if (!is_v) {
+    const __nv_bfloat16* wp = (is_q ? q_weight : k_weight) + lane * kPerLane;
+#pragma unroll
+    for (int i = 0; i < kPerLane; ++i) w[i] = __bfloat162float(wp[i]);
+  }
+  pdl_launch_dependents();  // consumer prologues (weight / KV prefetch) may start now
+  pdl_wait();
+  Vec* ptr = reinterpret_cast<Vec*>(qkv + ((int64_t)tok * heads + head) * kHeadDim) + lane;
+  const int64_t slot = slot_ids[tok];
+  const int kvh = is_v ? head - num_heads_q - num_heads_kv : head - num_heads_q;
+  const int64_t crow = (slot * num_heads_kv + kvh) * kHeadDim;
+  if (is_v) {
+    if (slot >= 0) reinterpret_cast<Vec*>(value_cache + crow)[lane] = *ptr;
+    return;
+  }
+  const Vec x = *ptr;
+  const uint32_t* xp = reinterpret_cast<const uint32_t*>(&x);
+  float e[kPerLane];
+#pragma unroll
+  for (int j = 0; j < kPerLane / 2; ++j) {
+    e[2 * j] = bf16lo(xp[j]);
+    e[2 * j + 1] = bf16hi(xp[j]);
+  }
+  qk_norm_rope_warp<kHeadDim, false>(e, w, eps, cos_sin_cache + positions[tok] * kHeadDim, kHeadDim, lane);
+  Vec y;
+  uint32_t* yp = reinterpret_cast<uint32_t*>(&y);
+#pragma unroll
+  for (int j = 0; j < kPerLane / 2; ++j) yp[j] = pack_bf16x2(e[2 * j], e[2 * j + 1]);
+  *ptr = y;
+  if (!is_q && slot >= 0) reinterpret_cast<Vec*>(key_cache + crow)[lane] = y;
   pdl_launch_dependents();
 }
 
@@ -734,6 +759,36 @@ extern "C" int xb_fused_qk_norm_rope_bf16(void* qkv, int num_heads_q, int num_he
   else if (head_dim == 128) { if (interleaved) XB_QKNR(128, true); else XB_QKNR(128, false); }
   else { if (interleaved) XB_QKNR(256, true); else XB_QKNR(256, false); }
 #undef XB_QKNR
+  return 0;
+}
+
+extern "C" int xb_qk_norm_rope_and_cache_bf16(void* qkv, int num_heads_q, int num_heads_kv, int head_dim, float eps,
+                                              const void* q_weight, const void* k_weight, const void* cos_sin_cache,
+                                              const int64_t* positions, const int32_t* slot_ids, void* key_cache,
+                                              void* value_cache, int num_tokens, xb_stream_t stream) {
+  XB_CHECK(head_dim == 64 || head_dim == 128, "qk_norm_rope_and_cache: head_dim %d unsupported (64 or 128)", head_dim);
+  XB_CHECK(num_heads_q > 0 && num_heads_kv > 0 && num_tokens >= 0, "qk_norm_rope_and_cache: bad heads %d/%d or tokens %d",
+           num_heads_q, num_heads_kv, num_tokens);
+  XB_CHECK(q_weight && k_weight && cos_sin_cache, "qk_norm_rope_and_cache: null q_weight, k_weight or cos_sin_cache");
+  if (num_tokens == 0) return 0;
+  XB_CHECK(qkv && positions && slot_ids && key_cache && value_cache, "qk_norm_rope_and_cache: null pointer argument");
+  const uintptr_t align = (uintptr_t)head_dim / 16;   // one 4- / 8-byte access per lane
+  XB_CHECK((reinterpret_cast<uintptr_t>(qkv) | reinterpret_cast<uintptr_t>(key_cache) |
+            reinterpret_cast<uintptr_t>(value_cache)) % align == 0,
+           "qk_norm_rope_and_cache: qkv and caches must be %d-byte aligned", (int)align);
+  const int64_t warps = (int64_t)num_tokens * (num_heads_q + 2 * num_heads_kv);
+  const int wpb = 8;
+  XB_CHECK(warps <= (int64_t)INT32_MAX - wpb, "qk_norm_rope_and_cache: %lld (token, head) pairs", (long long)warps);
+  dim3 grid((unsigned)((warps + wpb - 1) / wpb)), block(wpb * 32);
+  auto* p = reinterpret_cast<__nv_bfloat16*>(qkv);
+  auto* qw = reinterpret_cast<const __nv_bfloat16*>(q_weight);
+  auto* kw = reinterpret_cast<const __nv_bfloat16*>(k_weight);
+  auto* cs = reinterpret_cast<const __nv_bfloat16*>(cos_sin_cache);
+  auto* kc = reinterpret_cast<__nv_bfloat16*>(key_cache);
+  auto* vc = reinterpret_cast<__nv_bfloat16*>(value_cache);
+  auto kern = head_dim == 64 ? qk_norm_rope_and_cache_kernel<64> : qk_norm_rope_and_cache_kernel<128>;
+  XB_CUDA_OK(launch(kern, grid, block, 0, (cudaStream_t)stream, true, p, num_heads_q, num_heads_kv, eps, qw, kw, cs,
+                    positions, slot_ids, kc, vc, num_tokens));
   return 0;
 }
 

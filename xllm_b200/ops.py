@@ -182,6 +182,23 @@ def fused_qk_norm_rope(qkv, num_heads_q, num_heads_k, num_heads_v, head_dim, eps
                                            _p(position_ids), c_i32(T), _stream()), "fused_qk_norm_rope")
 
 
+def qk_norm_rope_and_cache(qkv, num_heads_q, num_heads_kv, head_dim, eps, q_weight, k_weight, cos_sin_cache, position_ids,
+                           slot_ids, key_cache, value_cache) -> None:
+    """Fused K10+K12 (one launch): per-head RMSNorm + NeoX RoPE of q and k in place in qkv [T, (Hq+2Hkv)*D], then the new
+    k and v rows into the paged caches (slot < 0 skipped); bit-identical to fused_qk_norm_rope + reshape_paged_cache."""
+    _cuda_bf16(qkv, "qkv"); _cuda_bf16(key_cache, "key_cache"); _cuda_bf16(value_cache, "value_cache")
+    _need(qkv.is_contiguous(), "qkv must be contiguous")
+    _need(key_cache.is_contiguous() and value_cache.is_contiguous(), "caches must be contiguous")
+    _need(position_ids.dtype == torch.int64, "position_ids must be int64")
+    _need(slot_ids.dtype == torch.int32, "slot_ids must be int32")
+    _need(cos_sin_cache.size(-1) == head_dim, "full rotary only (cos_sin_cache rows of head_dim)")
+    T = qkv.size(0)
+    check(lib().xb_qk_norm_rope_and_cache_bf16(_p(qkv), c_i32(num_heads_q), c_i32(num_heads_kv), c_i32(head_dim), c_f32(eps),
+                                               _p(q_weight), _p(k_weight), _p(cos_sin_cache), _p(position_ids),
+                                               _p(slot_ids), _p(key_cache), _p(value_cache), c_i32(T), _stream()),
+          "qk_norm_rope_and_cache")
+
+
 # ---- K11 --------------------------------------------------------------------
 _ACT = {"silu": 0, "gelu": 1, "gelu_tanh": 2, "gelu_pytorch_tanh": 2}
 

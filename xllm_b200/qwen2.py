@@ -45,6 +45,8 @@ class Qwen2Config:
     # models/llm/npu/llama.h:341-346, but builds its table from rope_theta alone, :77-106; the CUDA registry entry of
     # integration/patches/0002 applies them.)
     rope_scaling: Optional[dict] = None
+    # Qwen3: per-head RMSNorm of q and k (weights q_norm / k_norm [head_dim]) before RoPE (qwen2_attention.cpp:147-171)
+    qk_norm: bool = False
     name: str = "Qwen2-7B"
 
     @staticmethod
@@ -67,6 +69,24 @@ class Qwen2Config:
         d = dict(hidden_size=8192, num_layers=80, n_heads=64, n_kv_heads=8, head_dim=128, intermediate_size=28672,
                  vocab_size=128256, rope_theta=500000.0, rms_norm_eps=1e-5, quant="fp8", qkv_bias=False,
                  max_position_embeddings=8192, name="Llama-3-70B")
+        d.update(kw)
+        return Qwen2Config(**d)
+
+    @staticmethod
+    def qwen3_8b(**kw):
+        """Qwen3-8B (published config.json): head_dim 128 is not hidden / n_heads; no qkv bias, QK-norm."""
+        d = dict(hidden_size=4096, num_layers=36, n_heads=32, n_kv_heads=8, head_dim=128, intermediate_size=12288,
+                 vocab_size=151936, rope_theta=1000000.0, rms_norm_eps=1e-6, max_position_embeddings=40960,
+                 qkv_bias=False, qk_norm=True, name="Qwen3-8B")
+        d.update(kw)
+        return Qwen2Config(**d)
+
+    @staticmethod
+    def qwen3_0_6b(**kw):
+        """Qwen3-0.6B (published config.json): q_size 2048 over hidden 1024, tied embeddings."""
+        d = dict(hidden_size=1024, num_layers=28, n_heads=16, n_kv_heads=8, head_dim=128, intermediate_size=3072,
+                 vocab_size=151936, rope_theta=1000000.0, rms_norm_eps=1e-6, max_position_embeddings=40960,
+                 qkv_bias=False, qk_norm=True, tie_word_embeddings=True, name="Qwen3-0.6B")
         d.update(kw)
         return Qwen2Config(**d)
 
@@ -187,9 +207,13 @@ class Qwen2Weights:
                 post_norm=(1.0 + 0.05 * torch.randn(H, generator=g_rep, device=device)).to(BF16),
                 qkv=mk(q_size + 2 * kv_size, H, cfg.qkv_bias), o=mk(H, q_size),
                 gate_up=mk(2 * I, H), down=mk(H, I)))
-            # synthetic packed nibbles are random anyway: declare the gate_up rows interleaved so the fused epilogue runs
+            if cfg.qk_norm:
+                w.layers[-1]["q_norm"] = (1.0 + 0.05 * torch.randn(cfg.head_dim, generator=g_rep, device=device)).to(BF16)
+                w.layers[-1]["k_norm"] = (1.0 + 0.05 * torch.randn(cfg.head_dim, generator=g_rep, device=device)).to(BF16)
+            # synthetic packed nibbles are random anyway: declare the gate_up rows interleaved so the fused epilogue runs.
+            # The rope-pair qkv order serves only the GEMV's RoPE epilogue, which cannot normalise a head: plain under qk_norm.
             w.layers[-1]["gate_up"].gate_up_interleaved = cfg.quant == "w4a16"
-            w.layers[-1]["qkv"].qkv_rope_packed = cfg.quant == "w4a16"
+            w.layers[-1]["qkv"].qkv_rope_packed = cfg.quant == "w4a16" and not cfg.qk_norm
         return w
 
     def weight_bytes(self):
@@ -241,7 +265,10 @@ class Qwen2DecodeRunner:
         fuse_gemv: W4A16 decode with batch <= 8 splits add+RMSNorm between the o / down epilogues and the qkv / gate_up
         prologues (5 launches per layer instead of 7).  OFF by default: the 200-launch step's small add+RMSNorm kernels
         overlap the next GEMV's weight prefetch under PDL, while folded into the GEMVs they sit on every CTA's critical path.  RoPE + KV scatter (qkv epilogue) and SiLU*mul (gate_up epilogue) ride in the
-        GEMVs either way."""
+        GEMVs either way.  Always off for qk_norm (Qwen3) configs: it needs the rope-pair packed qkv epilogue, which cannot
+        normalise a head.
+        fused_rope_cache: qk_norm configs run qk_norm_rope_and_cache (one launch) when True, fused_qk_norm_rope +
+        reshape_paged_cache when False; other configs rope_and_cache vs rotary_embedding + reshape_paged_cache."""
         self.cfg, self.w, self.B, self.device = cfg, weights, max_batch, device
         self.pg = pg if (pg is not None and pg.world_size > 1) else None
         self.tp = self.pg.world_size if self.pg else 1
@@ -295,7 +322,9 @@ class Qwen2DecodeRunner:
         import os
         if os.environ.get("XB_FUSE_GEMV") is not None:          # A/B measurements
             fuse_gemv = os.environ["XB_FUSE_GEMV"] != "0"
-        self.fuse_gemv = bool(fuse_gemv and w4 and B <= 8 and ops.w4a16_decode_fused_fits(B, H))
+        if cfg.qk_norm and any(L["qkv"].qkv_rope_packed for L in weights.layers):
+            raise ValueError("qk_norm needs the plain qkv weight layout: the rope-pair packed one cannot normalise a head")
+        self.fuse_gemv = bool(fuse_gemv and w4 and B <= 8 and ops.w4a16_decode_fused_fits(B, H) and not cfg.qk_norm)
         # post-attention add+RMSNorm folded into the gate_up GEMV's prologue only (XB_FUSE_MLP_NORM=1; experiment): the wide
         # gate_up launch hides the prologue (+0.5 us measured) while the separate add+norm kernel costs ~2.2 us
         self.fuse_mlp_norm = bool(os.environ.get("XB_FUSE_MLP_NORM", "0") != "0" and w4 and B <= 8 and
@@ -371,6 +400,18 @@ class Qwen2DecodeRunner:
                                    num_heads=self.nh, num_kv_heads=self.nkv, head_dim=cfg.head_dim)
             return
         assert norm_w is None
+        if cfg.qk_norm:
+            lin.forward(h, self.qkv)
+            if self.fused_rope_cache:
+                ops.qk_norm_rope_and_cache(self.qkv, self.nh, self.nkv, cfg.head_dim, cfg.rms_norm_eps, L["q_norm"], L["k_norm"],
+                                           self.cos_sin, self.positions, self.slots, self.k_caches[li], self.v_caches[li])
+            else:
+                ops.fused_qk_norm_rope(self.qkv, self.nh, self.nkv, self.nkv, cfg.head_dim, cfg.rms_norm_eps, L["q_norm"],
+                                       L["k_norm"], self.cos_sin, False, self.positions)
+                k, v = self.qkv[:, qs:qs + kvs], self.qkv[:, qs + kvs:]
+                ops.reshape_paged_cache(self.slots, k.view(-1, self.nkv, cfg.head_dim), v.view(-1, self.nkv, cfg.head_dim),
+                                        self.k_caches[li], self.v_caches[li])
+            return
         if packed:
             lin.forward(h, self.qkv_raw)
             ops.rope_and_cache_packed(self.positions, self.qkv_raw, self.qkv, self.cos_sin, self.slots, self.k_caches[li],

@@ -88,7 +88,12 @@ class Qwen2PrefillRunner:
         for li, L in enumerate(w.layers):
             q, k, v = qkv[:, :qs], qkv[:, qs:qs + kvs], qkv[:, qs + kvs:]
             # RoPE on q/k and the KV scatter of this chunk (flashinfer_attention.cpp:128-131 scatters before attending)
-            if L["qkv"].qkv_rope_packed:
+            if cfg.qk_norm:
+                # Qwen3: per-head q / k RMSNorm + RoPE in place, then the scatter; the ragged path reads the normalised k from qkv
+                L["qkv"].forward(h, qkv)
+                ops.qk_norm_rope_and_cache(qkv, self.nh, self.nkv, D, cfg.rms_norm_eps, L["q_norm"], L["k_norm"], self.cos_sin,
+                                           positions, slots, self.k_caches[li], self.v_caches[li])
+            elif L["qkv"].qkv_rope_packed:
                 # decode-layout weights (rows in rope-pair order): the GEMM output is un-permuted by the rope kernel
                 L["qkv"].forward(h, qkv_raw)
                 ops.rope_and_cache_packed(positions, qkv_raw, qkv, self.cos_sin, slots, self.k_caches[li], self.v_caches[li],
